@@ -156,6 +156,17 @@ template <typename T> NVL_DEV void store_dst_vec(T *base, size_t idx, size_t n, 
 /* ------------------------------------------------------------------ */
 /* reduction templates                                                 */
 /* ------------------------------------------------------------------ */
+/* complex element (UCC_DT_FLOAT32_COMPLEX / FLOAT64_COMPLEX): re, im interleaved, aligned like cuFloatComplex / cuDoubleComplex.
+ * It is its own accumulator: sums and products stay in the component precision, as cuCaddf / cuCmulf do in ec/cuda. */
+template <typename R> struct alignas(2 * sizeof(R)) nvl_complex { R re, im; };
+typedef nvl_complex<float> nvl_c64;
+typedef nvl_complex<double> nvl_c128;
+template <typename R> NVL_DEV nvl_complex<R> operator+(nvl_complex<R> a, nvl_complex<R> b) { return {a.re + b.re, a.im + b.im}; }
+template <typename R> NVL_DEV nvl_complex<R> operator*(nvl_complex<R> a, nvl_complex<R> b)
+{ return {a.re * b.re - a.im * b.im, a.re * b.im + a.im * b.re}; }
+template <typename T> struct IsComplex { static constexpr bool v = false; };
+template <typename R> struct IsComplex<nvl_complex<R>> { static constexpr bool v = true; };
+
 template <typename T> struct AccOf { typedef T type; };
 template <> struct AccOf<__half> { typedef float type; };
 template <> struct AccOf<__nv_bfloat16> { typedef float type; };
@@ -186,10 +197,12 @@ template <typename A> struct OpFn<NVL_OP_BXOR, A> { static NVL_DEV A f(A a, A b)
 template <typename A> struct IsIntAcc { static constexpr bool v = true; };
 template <> struct IsIntAcc<float> { static constexpr bool v = false; };
 template <> struct IsIntAcc<double> { static constexpr bool v = false; };
+template <typename R> struct IsIntAcc<nvl_complex<R>> { static constexpr bool v = false; };
 template <int OP, typename A> NVL_DEV A avg_scale(A x, float inv_n, int n)
 {
     if (OP != NVL_OP_AVG) return x;
     if constexpr (IsIntAcc<A>::v) return n > 1 ? (A)(x / (A)n) : x;
+    else if constexpr (IsComplex<A>::v) return {x.re * inv_n, x.im * inv_n}; /* both components by the factor f32 / f64 use */
     else return (A)(x * (A)inv_n);
 }
 
@@ -216,25 +229,32 @@ template <> struct IsFloatLike<double> { static constexpr bool v = true; };
 template <> struct IsFloatLike<__half> { static constexpr bool v = true; };
 template <> struct IsFloatLike<__nv_bfloat16> { static constexpr bool v = true; };
 
-/* run F<T,OP>::run(args...) for the runtime operator; bit/logic operators only exist for integer types */
+/* run F<T,OP>::run(args...) for the runtime operator; complex types have SUM / AVG / PROD only, bit/logic operators only exist
+ * for integer types */
 #define NVL_DISPATCH_OP(_T, _op, _CALL)                                                         \
     do {                                                                                        \
         switch (_op) {                                                                          \
         case NVL_OP_SUM: _CALL(_T, NVL_OP_SUM); break;                                          \
         case NVL_OP_AVG: _CALL(_T, NVL_OP_AVG); break;                                          \
         case NVL_OP_PROD: _CALL(_T, NVL_OP_PROD); break;                                        \
-        case NVL_OP_MAX: _CALL(_T, NVL_OP_MAX); break;                                          \
-        case NVL_OP_MIN: _CALL(_T, NVL_OP_MIN); break;                                          \
         default:                                                                                \
-            if constexpr (!IsFloatLike<_T>::v) {                                                \
+            if constexpr (!IsComplex<_T>::v) {                                                  \
                 switch (_op) {                                                                  \
-                case NVL_OP_LAND: _CALL(_T, NVL_OP_LAND); break;                                \
-                case NVL_OP_LOR: _CALL(_T, NVL_OP_LOR); break;                                  \
-                case NVL_OP_LXOR: _CALL(_T, NVL_OP_LXOR); break;                                \
-                case NVL_OP_BAND: _CALL(_T, NVL_OP_BAND); break;                                \
-                case NVL_OP_BOR: _CALL(_T, NVL_OP_BOR); break;                                  \
-                case NVL_OP_BXOR: _CALL(_T, NVL_OP_BXOR); break;                                \
-                default: break;                                                                 \
+                case NVL_OP_MAX: _CALL(_T, NVL_OP_MAX); break;                                  \
+                case NVL_OP_MIN: _CALL(_T, NVL_OP_MIN); break;                                  \
+                default:                                                                        \
+                    if constexpr (!IsFloatLike<_T>::v) {                                        \
+                        switch (_op) {                                                          \
+                        case NVL_OP_LAND: _CALL(_T, NVL_OP_LAND); break;                        \
+                        case NVL_OP_LOR: _CALL(_T, NVL_OP_LOR); break;                          \
+                        case NVL_OP_LXOR: _CALL(_T, NVL_OP_LXOR); break;                        \
+                        case NVL_OP_BAND: _CALL(_T, NVL_OP_BAND); break;                        \
+                        case NVL_OP_BOR: _CALL(_T, NVL_OP_BOR); break;                          \
+                        case NVL_OP_BXOR: _CALL(_T, NVL_OP_BXOR); break;                        \
+                        default: break;                                                         \
+                        }                                                                       \
+                    }                                                                           \
+                    break;                                                                      \
                 }                                                                               \
             }                                                                                   \
             break;                                                                              \

@@ -144,6 +144,8 @@ NVL_DEFINE_ENTRY(nvl_allreduce_oneshot_kernel, nvl_red_args_t)
 template <typename T, int OP> struct McRed { static __device__ __forceinline__ uint4 ld(const void *) { return make_uint4(0, 0, 0, 0); } };
 #define NVL_MCRED(_T, _OP, _fn) template <> struct McRed<_T, _OP> { static __device__ __forceinline__ uint4 ld(const void *p) { return _fn(p); } };
 NVL_MCRED(float, NVL_OP_SUM, mc_ld_reduce_f32) NVL_MCRED(float, NVL_OP_AVG, mc_ld_reduce_f32)
+/* complex float: re / im are interleaved floats, so the float vector sum is the complex sum */
+NVL_MCRED(nvl_c64, NVL_OP_SUM, mc_ld_reduce_f32) NVL_MCRED(nvl_c64, NVL_OP_AVG, mc_ld_reduce_f32)
 NVL_MCRED(__half, NVL_OP_SUM, mc_ld_reduce_f16) NVL_MCRED(__half, NVL_OP_AVG, mc_ld_reduce_f16)
 NVL_MCRED(__nv_bfloat16, NVL_OP_SUM, mc_ld_reduce_bf16) NVL_MCRED(__nv_bfloat16, NVL_OP_AVG, mc_ld_reduce_bf16)
 NVL_MCRED(int32_t, NVL_OP_SUM, mc_red_add_s32) NVL_MCRED(int32_t, NVL_OP_MIN, mc_red_min_s32) NVL_MCRED(int32_t, NVL_OP_MAX, mc_red_max_s32)

@@ -6,9 +6,11 @@ set -e
 cd "$(dirname "$0")/.."
 K=src/components/tl/nvl/kernels
 /usr/bin/g++ -O1 -g -fsanitize=thread -std=c++17 -pthread -I/usr/local/cuda/include -I$K -Iinclude -Isrc tests/emu/nvl_emu.cpp -o /tmp/ucc_b200_emu_tsan
+/usr/bin/g++ -O1 -g -fsanitize=thread -std=c++17 -pthread -I/usr/local/cuda/include -I$K -Iinclude -Isrc tests/emu/nvl_emu_complex.cpp -o /tmp/ucc_b200_emu_complex_tsan
 rc=0
-for w in staged xchg pipe symm push oneshot_rs soak soak2; do
-  TSAN_OPTIONS="halt_on_error=0:report_signal_unsafe=0" /tmp/ucc_b200_emu_tsan $w > /tmp/ucc_b200_emu_tsan_$w.log 2>&1 || true
+for w in staged xchg pipe symm push oneshot_rs soak soak2 complex; do
+  exe=/tmp/ucc_b200_emu_tsan; [ "$w" = complex ] && exe=/tmp/ucc_b200_emu_complex_tsan   # (complex float / double kernels: own driver)
+  TSAN_OPTIONS="halt_on_error=0:report_signal_unsafe=0" $exe $w > /tmp/ucc_b200_emu_tsan_$w.log 2>&1 || true
   n=$(grep -c 'WARNING: ThreadSanitizer' /tmp/ucc_b200_emu_tsan_$w.log || true)
   ok=$(grep -c NVL_EMU_OK /tmp/ucc_b200_emu_tsan_$w.log || true)
   echo "$w: tsan reports $n, result $([ "$ok" = 1 ] && echo ok || echo FAILED)"
