@@ -140,6 +140,18 @@ typedef struct nvl_push_args {
     size_t         recv_off[NVL_MAX_PEERS];
 } nvl_push_args_t;
 
+/* in-place alltoall(v) as pairwise swaps (kernels/nvl_swap.cu): my region for member p = len[p] bytes at buf + off[p]; it trades
+ * contents with p's region for me inside dst_of[p] (p's buffer mapped here) */
+typedef struct nvl_swap_args {
+    nvl_team_dev_t team;
+    char          *buf;
+    char          *dst_of[NVL_MAX_PEERS];
+    size_t         off[NVL_MAX_PEERS], len[NVL_MAX_PEERS];
+    int            lookup;       /* alltoallv: every rank publishes (off[], len[]) at the start of its heap data region, one table per
+                                    block, and reads entry [rank] of each peer's; alltoall: p's region for me is (off[rank], len[rank]) */
+} nvl_swap_args_t;
+#define NVL_SWAP_TABLE_BYTES (2 * NVL_MAX_PEERS * sizeof(uint64_t)) /* per block */
+
 /* two-member active-set broadcast = send / recv (kernels/nvl_p2p.cu) */
 typedef struct nvl_p2p_args {
     nvl_team_dev_t team;
@@ -187,6 +199,7 @@ cudaError_t  nvl_launch_exchange(const nvl_xchg_args_t *a, int nblocks, int nthr
 cudaError_t  nvl_launch_exchange_push(const nvl_push_args_t *a, int nblocks, int nthreads, cudaStream_t s);
 /* same exchange driven by the TMA engine (cp.async.bulk through shared memory): one-warp CTAs */
 cudaError_t  nvl_launch_exchange_push_bulk(const nvl_push_args_t *a, int nblocks, cudaStream_t s);
+cudaError_t  nvl_launch_exchange_swap(const nvl_swap_args_t *a, int nblocks, int nthreads, cudaStream_t s);
 cudaError_t  nvl_launch_barrier(const nvl_team_dev_t *t, cudaStream_t s);
 cudaError_t  nvl_launch_self_copy(void *dst, const void *src, size_t bytes, int nblocks, int nthreads, cudaStream_t s); /* team of one */
 cudaError_t  nvl_launch_self_copy_bulk(void *dst, const void *src, size_t bytes, int nblocks, cudaStream_t s);      /* same, TMA engine; 16-byte aligned pointers */

@@ -221,6 +221,8 @@ typedef struct ucc_tl_nvl_task {
     int                 use_bulk;      /* push exchange driven by the TMA engine (nvl_exchange_push_bulk_kernel) */
     int                 use_ce;        /* push exchange executed by the copy engines (cudaMemcpyAsync between two barrier kernels) */
     int                 use_push;
+    int                 use_swap;      /* in-place alltoall(v): pairwise swap kernel (kernels/nvl_swap.cu) when the buffers resolved,
+                                          else the heap-staged pull (nvl_launch) */
     struct { size_t send_off[NVL_MAX_PEERS], send_bytes[NVL_MAX_PEERS], land_off[NVL_MAX_PEERS], recv_off[NVL_MAX_PEERS], peer_land[NVL_MAX_PEERS]; int lookup; } push;
 } ucc_tl_nvl_task_t;
 

@@ -11,6 +11,10 @@
 
 #define NVL_LIB(_t) ((_t)->super.super.context->lib)
 
+/* kernels/nvl_swap.cu, linked into the plugin.  Weak, so that a plugin linked with a launcher set that lacks it (the host-emulated
+ * plugin of tests/emu/build_hostemu.sh) still loads with immediate binding; such a plugin declines in-place alltoall(v) (xchg_init) */
+#pragma weak nvl_launch_exchange_swap
+
 static int to_nvl_dt(ucc_datatype_t dt)
 {
     switch (dt) {
@@ -52,7 +56,7 @@ static void note_launch(const ucc_tl_nvl_task_t *t)
     case NVL_TASK_REDUCE_PIPE: k = "nvls_pipe"; break;
     case NVL_TASK_REDUCE_SYMM: k = "nvls_symm_inplace"; break;
     case NVL_TASK_AG_SYMM: k = "allgather_symm_mc"; break;
-    case NVL_TASK_XCHG: k = (t->use_push && t->u.xchg.direct) ? (t->use_ce ? "exchange_push_copy_engine" : (t->use_bulk ? "exchange_push_bulk(tma)" : "exchange_push")) : (t->u.xchg.direct ? "exchange_pull_zcopy" : (t->u.xchg.use_mc ? "exchange_nvls" : (t->u.xchg.ring ? "exchange_ring" : "exchange_pull_staged"))); break;
+    case NVL_TASK_XCHG: k = t->use_swap ? (t->u.xchg.direct ? "exchange_swap" : "exchange_pull_staged_inplace") : (t->use_push && t->u.xchg.direct) ? (t->use_ce ? "exchange_push_copy_engine" : (t->use_bulk ? "exchange_push_bulk(tma)" : "exchange_push")) : (t->u.xchg.direct ? "exchange_pull_zcopy" : (t->u.xchg.use_mc ? "exchange_nvls" : (t->u.xchg.ring ? "exchange_ring" : "exchange_pull_staged"))); break;
     case NVL_TASK_SELF_COPY: k = t->use_bulk ? "self_copy_bulk(tma)" : "self_copy"; break;
     case NVL_TASK_P2P:
         if (t->u.p2p.mode == NVL_P2P_PUSH) { k = "p2p_send_rndv(push)"; nb = nvl_p2p_push_ctas(t->u.p2p.bytes); }
@@ -62,6 +66,31 @@ static void note_launch(const ucc_tl_nvl_task_t *t)
     default: nb = 1; break;
     }
     snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", k, nb, (t->use_bulk && !t->use_ce && (t->kind == NVL_TASK_SELF_COPY || (t->use_push && t->u.xchg.direct))) ? 32 : t->nthreads);
+}
+
+/* in-place alltoall(v).  Buffers resolved: one swap kernel trades every pair of regions between the mapped buffers.  Otherwise my
+ * buffer is first copied into my heap's staging area, and the pull kernel reads the peers' staging areas through its `direct`
+ * tables.  The pull kernel's own staging phase cannot run in place: its barrier orders my blocks against the peers' blocks only,
+ * so one of my blocks could overwrite a region that another of my blocks is still staging. */
+static cudaError_t launch_swap(ucc_tl_nvl_task_t *t, cudaStream_t s)
+{
+    nvl_xchg_args_t x = t->u.xchg;
+    const int N = x.team.size, me = x.team.rank;
+    cudaError_t e;
+    if (x.direct) {
+        nvl_swap_args_t sa;
+        memset(&sa, 0, sizeof(sa));
+        sa.team = x.team; sa.buf = (char *)x.dst; sa.lookup = x.publish_table;
+        for (int p = 0; p < N; p++) { sa.dst_of[p] = x.d.dst[p]; sa.off[p] = x.dst_off[p]; sa.len[p] = x.pull_bytes[p]; }
+        return nvl_launch_exchange_swap(&sa, t->nblocks, t->nthreads, s);
+    }
+    if (x.src_bytes) {
+        e = nvl_launch_self_copy(x.team.heap[me] + NVL_DATA_OFFSET + NVL_XCHG_TABLE_BYTES, x.src, x.src_bytes, t->nblocks, t->nthreads, s);
+        if (e != cudaSuccess) return e;
+    }
+    x.direct = 1;
+    for (int p = 0; p < N; p++) x.d.src[p] = x.team.heap[p] + NVL_DATA_OFFSET + NVL_XCHG_TABLE_BYTES;
+    return nvl_launch_exchange(&x, t->nblocks, t->nthreads, s);
 }
 
 static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
@@ -82,7 +111,8 @@ static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
     case NVL_TASK_REDUCE_SYMM: e = nvl_launch_reduce_symm(&t->u.red, t->nblocks, t->nthreads, s); break;
     case NVL_TASK_AG_SYMM: e = nvl_launch_allgather_symm(&t->u.xchg, t->nblocks, t->nthreads, s); break;
     case NVL_TASK_XCHG:
-        if (t->use_push && t->u.xchg.direct) { /* every member's destination resolved: store my blocks straight into them */
+        if (t->use_swap) e = launch_swap(t, s);
+        else if (t->use_push && t->u.xchg.direct) { /* every member's destination resolved: store my blocks straight into them */
             nvl_push_args_t pa;
             memset(&pa, 0, sizeof(pa));
             pa.team = t->u.xchg.team; pa.src = t->u.xchg.src;
@@ -565,7 +595,7 @@ static ucc_status_t task_alloc(ucc_base_coll_args_t *b, ucc_base_team_t *b_team,
     ucc_tl_nvl_task_t *t = (ucc_tl_nvl_task_t *)ucc_mpool_get(&ctx->task_mp);
     if (!t) return UCC_ERR_NO_MEMORY;
     ucc_coll_task_init(&t->super, b, b_team);
-    t->team = team; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->want_direct = 0; t->gated = 0; t->use_push = 0; t->use_bulk = 0; t->use_ce = 0;
+    t->team = team; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->want_direct = 0; t->gated = 0; t->use_push = 0; t->use_bulk = 0; t->use_ce = 0; t->use_swap = 0;
     t->need_xchg = 0; t->direct_cached = 0; t->cached_mode = 0; t->need_src = t->need_dst = 0; t->exp_src = NULL; t->exp_dst = NULL; t->exp_src_len = t->exp_dst_len = 0; t->nblocks_direct = 0;
     t->nthreads = (int)ctx->cfg.nthreads;
     t->super.post = nvl_post; t->super.progress = nvl_progress; t->super.finalize = nvl_finalize; t->super.triggered_post = nvl_triggered_post;
@@ -797,6 +827,7 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     size_t moved = 0, dts;
     ucc_status_t st;
     if (team->self) return self_init(b, b_team, task_p);
+    if (inplace && (a->coll_type == UCC_COLL_TYPE_ALLTOALL || a->coll_type == UCC_COLL_TYPE_ALLTOALLV) && !nvl_launch_exchange_swap) return UCC_ERR_NOT_SUPPORTED;
     memset(&x, 0, sizeof(x));
     x.team = team->dev;
     if (UCC_COLL_ARGS_ACTIVE_SET(a)) {
@@ -849,18 +880,18 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
         break; }
     case UCC_COLL_TYPE_ALLTOALL: {
         size_t blk = a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype);
-        if (inplace) return UCC_ERR_NOT_SUPPORTED; /* would need a full private copy: leave to the fallback TL */
-        if (!is_cuda(a->dst.info.mem_type) || !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info.buffer; x.src = a->src.info.buffer; x.src_bytes = blk * N; x.self_off = me * blk;
+        if (!is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
+        x.dst = a->dst.info.buffer; x.src = inplace ? x.dst : a->src.info.buffer; x.src_bytes = blk * N; x.self_off = me * blk;
         for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = me * blk; x.pull_bytes[p] = blk; x.dst_off[p] = p * blk; }
         moved = blk * N; break; }
     case UCC_COLL_TYPE_ALLTOALLV: {
-        size_t sdt = ucc_dt_size(a->src.info_v.datatype), ddt = ucc_dt_size(a->dst.info_v.datatype), end = 0;
-        if (inplace) return UCC_ERR_NOT_SUPPORTED;
-        if (!is_cuda(a->dst.info_v.mem_type) || !is_cuda(a->src.info_v.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info_v.buffer; x.src = a->src.info_v.buffer; x.publish_table = 1;
+        /* in place: the dst counts / displacements describe my buffer in both directions */
+        const ucc_coll_buffer_info_v_t *sv = inplace ? &a->dst.info_v : &a->src.info_v;
+        size_t sdt = ucc_dt_size(sv->datatype), ddt = ucc_dt_size(a->dst.info_v.datatype), end = 0;
+        if (!is_cuda(a->dst.info_v.mem_type) || !is_cuda(sv->mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        x.dst = a->dst.info_v.buffer; x.src = sv->buffer; x.publish_table = 1;
         for (ucc_rank_t p = 0; p < N; p++) {
-            size_t so = ucc_coll_args_get_displacement(a, a->src.info_v.displacements, p) * sdt, sc = ucc_coll_args_get_count(a, a->src.info_v.counts, p) * sdt;
+            size_t so = ucc_coll_args_get_displacement(a, sv->displacements, p) * sdt, sc = ucc_coll_args_get_count(a, sv->counts, p) * sdt;
             x.stage_off[p] = so; if (so + sc > end) end = so + sc;
             x.pull_off[p] = NVL_XCHG_LOOKUP; x.pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * ddt;
             x.dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * ddt; moved += x.pull_bytes[p];
@@ -918,7 +949,18 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
      * scatterv `moved` is private to a rank: use a fixed grid for those */
     if (a->coll_type == UCC_COLL_TYPE_ALLTOALLV || a->coll_type == UCC_COLL_TYPE_GATHERV || a->coll_type == UCC_COLL_TYPE_SCATTERV)
         t->nblocks = (int)ucc_min(ctx->cfg.max_blocks, (ctx->cfg.nblocks != UCC_UUNITS_AUTO && ctx->cfg.nblocks > 0) ? ctx->cfg.nblocks : 128u);
-    if (team->zcopy && ctx->cfg.zcopy != UCC_NO) {
+    if (inplace && (a->coll_type == UCC_COLL_TYPE_ALLTOALL || a->coll_type == UCC_COLL_TYPE_ALLTOALLV)) {
+        /* the buffers travel over the exchange board (or come from registrations) as destinations: the swap kernel reads and
+         * writes them in place, and when they do not resolve, launch_swap stages.  The zero-copy pull (need_src) must never run
+         * in place: the peers overwrite the buffer it reads. */
+        t->use_swap = 1;
+        if (ctx->cfg.zcopy != UCC_NO && (size_t)t->nblocks * NVL_SWAP_TABLE_BYTES <= ctx->cfg.symmetric_size) {
+            t->want_direct = NVL_DIRECT_FULL; t->need_src = 0; t->need_dst = 1;
+            t->exp_dst = x.dst; t->exp_dst_len = x.src_bytes;
+            memh_direct(t, a, NULL, x.dst);
+            if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
+        }
+    } else if (team->zcopy && ctx->cfg.zcopy != UCC_NO) {
         /* `moved` is the same number on every rank except for the v-collectives whose counts are private to a
          * rank (alltoallv, gatherv, scatterv): those only go zero-copy when it is forced, size-independently */
         int symmetric = a->coll_type != UCC_COLL_TYPE_ALLTOALLV && a->coll_type != UCC_COLL_TYPE_GATHERV && a->coll_type != UCC_COLL_TYPE_SCATTERV;
@@ -948,7 +990,7 @@ static ucc_status_t xchg_init_push(ucc_base_coll_args_t *b, ucc_base_team_t *b_t
     ucc_status_t st;
     if (ct != UCC_COLL_TYPE_ALLGATHER && ct != UCC_COLL_TYPE_ALLGATHERV && ct != UCC_COLL_TYPE_ALLTOALL && ct != UCC_COLL_TYPE_ALLTOALLV) return UCC_ERR_NOT_SUPPORTED;
     if (!team->self && (!team->zcopy || ctx->cfg.zcopy == UCC_NO)) return UCC_ERR_NOT_SUPPORTED;
-    if (ct == UCC_COLL_TYPE_ALLTOALL && UCC_IS_INPLACE(*a)) return UCC_ERR_NOT_SUPPORTED;
+    if ((ct == UCC_COLL_TYPE_ALLTOALL || ct == UCC_COLL_TYPE_ALLTOALLV) && UCC_IS_INPLACE(*a)) return UCC_ERR_NOT_SUPPORTED; /* -> swap, through the score fallback */
     st = xchg_init(b, b_team, task_p);
     if (st != UCC_OK) return st;
     t = ucc_derived_of(*task_p, ucc_tl_nvl_task_t); x = &t->u.xchg;
@@ -990,6 +1032,13 @@ static ucc_status_t xchg_init_ce(ucc_base_coll_args_t *b, ucc_base_team_t *b_tea
     if (t->kind != NVL_TASK_XCHG) return UCC_OK;
     t->use_ce = 1; t->use_bulk = 0; t->nblocks = 1;
     return UCC_OK;
+}
+
+/* in-place alltoall(v) only (kernels/nvl_swap.cu): what `pull` also does with such a request, under a name TUNE can select */
+static ucc_status_t xchg_init_swap(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
+{
+    if (!UCC_IS_INPLACE(b->args)) return UCC_ERR_NOT_SUPPORTED;
+    return xchg_init(b, b_team, task_p);
 }
 
 /* allgather(v) / bcast through the switch: every rank multicasts its block once (multimem.st), everybody then
@@ -1081,7 +1130,8 @@ static const nvl_alg_t algs_ag[] = {{"pull", "stage once, every peer pulls its p
     {"ce", "zero-copy push by the copy engines: cudaMemcpyAsync into the members' mapped destinations between two barrier kernels", xchg_init_ce}, {NULL}};
 static const nvl_alg_t algs_a2a[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init},
     {"push", "zero-copy push: every rank stores block p straight into member p's mapped destination; alltoallv looks the landing offset up in a table the receiver publishes on the device", xchg_init_push},
-    {"ce", "zero-copy push by the copy engines (reference ALLTOALL_USE_COPY_ENGINE): one cudaMemcpyAsync per peer between two barrier kernels", xchg_init_ce}, {NULL}};
+    {"ce", "zero-copy push by the copy engines (reference ALLTOALL_USE_COPY_ENGINE): one cudaMemcpyAsync per peer between two barrier kernels", xchg_init_ce},
+    {"swap", "in place only: every pair of members swaps its two regions straight between their mapped buffers, no staging (staged pull when a buffer cannot be mapped)", xchg_init_swap}, {NULL}};
 static const nvl_alg_t algs_barrier[] = {{"flags", "flag exchange in peer memory", barrier_init}, {NULL}};
 static const nvl_alg_t *const nvl_algs[UCC_COLL_TYPE_NUM] = {
     algs_ag, algs_ag, algs_allreduce, algs_a2a, algs_a2a, algs_barrier, algs_xchg_mc, algs_barrier, algs_barrier,

@@ -141,15 +141,26 @@ def reduce_scatter_tensor(output, input, op="sum", comm=None, async_op=False):
 def all_to_all_single(output, input, output_split_sizes=None, input_split_sizes=None, comm=None, async_op=False):
     """Equal splits -> alltoall; explicit split sizes (in elements of dim 0 rows) -> alltoallv (MoE dispatch / combine)."""
     comm = comm or default_comm()
+    return _launch(comm, _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes), input, async_op)
+
+
+def _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes):
+    """alltoall / alltoallv request; `output` and `input` being the same memory makes it an in-place request, whose counts and
+    displacements are those of the output (an in-place alltoallv needs the same split sizes in both directions)"""
+    inplace = output.data_ptr() == input.data_ptr()
+    src = None if inplace else input
     if output_split_sizes is None and input_split_sizes is None:
-        return _launch(comm, comm.coll_init("alltoall", input, output), input, async_op)
+        return comm.coll_init("alltoall", src, output, inplace=inplace)
     row = input[0].numel() if input.dim() > 1 else 1
     sc = [int(s) * row for s in input_split_sizes]
     rc = [int(s) * row for s in output_split_sizes]
     sd = [sum(sc[:i]) for i in range(len(sc))]
     rd = [sum(rc[:i]) for i in range(len(rc))]
-    req = comm.coll_init("alltoallv", input, output, src_counts=sc, src_displs=sd, dst_counts=rc, dst_displs=rd)
-    return _launch(comm, req, input, async_op)
+    if inplace:
+        if sc != rc:
+            raise ValueError("in-place all_to_all_single needs input_split_sizes == output_split_sizes")
+        return comm.coll_init("alltoallv", None, output, inplace=True, dst_counts=rc, dst_displs=rd)
+    return comm.coll_init("alltoallv", input, output, src_counts=sc, src_displs=sd, dst_counts=rc, dst_displs=rd)
 
 
 def all_gather_v(output, input, counts, comm=None, async_op=False):

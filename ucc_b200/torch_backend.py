@@ -15,6 +15,7 @@ import torch
 import torch.distributed as dist
 
 from .dist import Communicator
+from .ops import _alltoall_init
 
 _OPS = {dist.ReduceOp.SUM: "sum", dist.ReduceOp.PRODUCT: "prod", dist.ReduceOp.MIN: "min", dist.ReduceOp.MAX: "max", dist.ReduceOp.AVG: "avg",
         dist.ReduceOp.BAND: "band", dist.ReduceOp.BOR: "bor", dist.ReduceOp.BXOR: "bxor"}
@@ -164,12 +165,9 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         return w
 
     def alltoall_base(self, output, input, output_split_sizes, input_split_sizes, opts=None):
-        if not output_split_sizes and not input_split_sizes:
-            return self._run([self._comm.coll_init("alltoall", input.contiguous(), output)], [input], output)
-        row = input[0].numel() if input.dim() > 1 else 1
-        sc = [int(s) * row for s in input_split_sizes]; rc = [int(s) * row for s in output_split_sizes]
-        sd = [sum(sc[:i]) for i in range(len(sc))]; rd = [sum(rc[:i]) for i in range(len(rc))]
-        req = self._comm.coll_init("alltoallv", input.contiguous(), output, src_counts=sc, src_displs=sd, dst_counts=rc, dst_displs=rd)
+        # an output aliasing the input makes it an in-place request
+        equal = not output_split_sizes and not input_split_sizes
+        req = _alltoall_init(self._comm, output, input.contiguous(), None if equal else output_split_sizes, None if equal else input_split_sizes)
         return self._run([req], [input], output)
 
     # ---- point to point: a two-member active-set broadcast, exactly how ProcessGroupUCC maps send/recv onto UCC.
