@@ -202,7 +202,6 @@ cudaError_t  nvl_launch_exchange_push_bulk(const nvl_push_args_t *a, int nblocks
 cudaError_t  nvl_launch_exchange_swap(const nvl_swap_args_t *a, int nblocks, int nthreads, cudaStream_t s);
 cudaError_t  nvl_launch_barrier(const nvl_team_dev_t *t, cudaStream_t s);
 cudaError_t  nvl_launch_self_copy(void *dst, const void *src, size_t bytes, int nblocks, int nthreads, cudaStream_t s); /* team of one */
-cudaError_t  nvl_launch_self_copy_bulk(void *dst, const void *src, size_t bytes, int nblocks, cudaStream_t s);      /* same, TMA engine; 16-byte aligned pointers */
 cudaError_t  nvl_launch_ctrl_init(void *heap_base, cudaStream_t s);
 #ifdef __cplusplus
 }

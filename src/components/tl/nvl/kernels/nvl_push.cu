@@ -96,24 +96,6 @@ __global__ void __launch_bounds__(32) nvl_exchange_push_bulk_kernel(const __grid
     bs.wait_all_blocks(t, 2);
     bs.finish(2);
 }
-/* team of one / plain device copy with the TMA engine: every CTA streams its chunks through the shared-memory ring */
-__global__ void __launch_bounds__(32) nvl_self_copy_bulk_kernel(char *dst, const char *src, size_t n)
-{
-    extern __shared__ __align__(128) char bulk_smem[];
-    if (threadIdx.x == 0) {
-        BulkPipe pp; pp.init(bulk_smem);
-        bulk_copy_range(pp, dst, src, n & ~(size_t)15, blockIdx.x, gridDim.x, 0);
-        bulk_wait_all();
-    }
-    if (blockIdx.x == 0) for (size_t i = (n & ~(size_t)15) + threadIdx.x; i < n; i += 32) dst[i] = src[i];
-}
-extern "C" cudaError_t nvl_launch_self_copy_bulk(void *dst, const void *src, size_t bytes, int nblocks, cudaStream_t s)
-{
-    static int attr_set = 0;
-    if (!attr_set) { cudaError_t e = cudaFuncSetAttribute(nvl_self_copy_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, NVL_BULK_SMEM); if (e != cudaSuccess) return e; attr_set = 1; }
-    nvl_self_copy_bulk_kernel<<<nblocks, 32, NVL_BULK_SMEM, s>>>(static_cast<char *>(dst), static_cast<const char *>(src), bytes);
-    return cudaGetLastError();
-}
 extern "C" cudaError_t nvl_launch_exchange_push_bulk(const nvl_push_args_t *a, int nblocks, cudaStream_t s)
 {
     static int attr_set = 0;

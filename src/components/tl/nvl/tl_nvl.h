@@ -219,7 +219,7 @@ typedef struct ucc_tl_nvl_task {
     nvl_xb_buf_t        rz_buf;        /* recv: what will be published */
     /* zero-copy push exchange (kernels/nvl_push.cu): used instead of the pull kernel when the destinations resolved */
     int                 use_bulk;      /* push exchange driven by the TMA engine (nvl_exchange_push_bulk_kernel) */
-    int                 use_ce;        /* push exchange executed by the copy engines (cudaMemcpyAsync between two barrier kernels) */
+    int                 use_ce;        /* push exchange executed by the copy engines (cudaMemcpyAsync between two barrier kernels); team of one: the copy is one cudaMemcpyAsync */
     int                 use_push;
     int                 use_swap;      /* in-place alltoall(v): pairwise swap kernel (kernels/nvl_swap.cu) when the buffers resolved,
                                           else the heap-staged pull (nvl_launch) */

@@ -57,7 +57,9 @@ static void note_launch(const ucc_tl_nvl_task_t *t)
     case NVL_TASK_REDUCE_SYMM: k = "nvls_symm_inplace"; break;
     case NVL_TASK_AG_SYMM: k = "allgather_symm_mc"; break;
     case NVL_TASK_XCHG: k = t->use_swap ? (t->u.xchg.direct ? "exchange_swap" : "exchange_pull_staged_inplace") : (t->use_push && t->u.xchg.direct) ? (t->use_ce ? "exchange_push_copy_engine" : (t->use_bulk ? "exchange_push_bulk(tma)" : "exchange_push")) : (t->u.xchg.direct ? "exchange_pull_zcopy" : (t->u.xchg.use_mc ? "exchange_nvls" : (t->u.xchg.ring ? "exchange_ring" : "exchange_pull_staged"))); break;
-    case NVL_TASK_SELF_COPY: k = t->use_bulk ? "self_copy_bulk(tma)" : "self_copy"; break;
+    case NVL_TASK_SELF_COPY:
+        if (t->use_ce) { snprintf(nvl_last_launch, sizeof(nvl_last_launch), "self_copy(cudaMemcpyAsync)"); return; }   /* no grid */
+        k = "self_copy"; break;
     case NVL_TASK_P2P:
         if (t->u.p2p.mode == NVL_P2P_PUSH) { k = "p2p_send_rndv(push)"; nb = nvl_p2p_push_ctas(t->u.p2p.bytes); }
         else if (t->u.p2p.mode == NVL_P2P_WAIT) { k = "p2p_recv_rndv(wait)"; nb = 1; }
@@ -65,7 +67,7 @@ static void note_launch(const ucc_tl_nvl_task_t *t)
         break;
     default: nb = 1; break;
     }
-    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", k, nb, (t->use_bulk && !t->use_ce && (t->kind == NVL_TASK_SELF_COPY || (t->use_push && t->u.xchg.direct))) ? 32 : t->nthreads);
+    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", k, nb, (t->use_bulk && !t->use_ce && t->use_push && t->u.xchg.direct) ? 32 : t->nthreads);
 }
 
 /* in-place alltoall(v).  Buffers resolved: one swap kernel trades every pair of regions between the mapped buffers.  Otherwise my
@@ -143,7 +145,7 @@ static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
     case NVL_TASK_P2P: e = nvl_launch_p2p(&t->u.p2p, t->nthreads, s); break;
     case NVL_TASK_SELF_COPY:
         if (!t->u.xchg.src_bytes) e = cudaSuccess;
-        else if (t->use_bulk) e = nvl_launch_self_copy_bulk(t->u.xchg.dst, t->u.xchg.src, t->u.xchg.src_bytes, t->nblocks, s);
+        else if (t->use_ce) e = cudaMemcpyAsync(t->u.xchg.dst, t->u.xchg.src, t->u.xchg.src_bytes, cudaMemcpyDeviceToDevice, s);
         else e = nvl_launch_self_copy(t->u.xchg.dst, t->u.xchg.src, t->u.xchg.src_bytes, t->nblocks, t->nthreads, s);
         break;
     default: e = nvl_launch_barrier(&t->u.red.team, s); break;
@@ -656,12 +658,12 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     t->kind = NVL_TASK_SELF_COPY;
     t->u.xchg.src = src; t->u.xchg.dst = dst; t->u.xchg.src_bytes = (src && dst && src != dst) ? bytes : 0;
     t->nblocks = pick_blocks(ctx, bytes, 64 * 1024);
-    /* big copies: the TMA engine streams them through shared memory, one one-warp CTA per SM (tools/exp_selfcopy.py; H100 SXM
-     * 80 GB at a 400 W limit, 1 GiB: 734 us, against 786 us on every second SM and 752 us for 256 x 512 copying threads); below
-     * ~128 MB the thread copy is as fast */
-    if (ctx->cfg.bulk != UCC_NO && t->u.xchg.src_bytes >= ((size_t)128 << 20) && !((((uintptr_t)src) | ((uintptr_t)dst)) & 15)) {
-        t->use_bulk = 1; t->nblocks = (int)ucc_max(1u, ucc_min((unsigned)ctx->sm_count, ctx->cfg.max_blocks));
-    }
+    /* from 16 MB up, cudaMemcpyAsync is the fastest copy measured (tools/selfcopy_study.py, H100 SXM 80 GB HBM3 at a 700 W
+     * limit, medians of 7 rounds of 20 copies): 1 GiB 709.8 us, against 713.8 us for the best kernel candidate (non-persistent
+     * TMA ring, 16 KB x 4 stages, 4 chunks per CTA), 715.5 us for the best thread copy and 732.3 us for the former persistent
+     * TMA ring; 64 MB 47.7 us against 49.7 us for the thread copy below; 16 MB 8.9 us against 11.1 us.  Smaller copies, not
+     * measured against it, keep the thread copy. */
+    if (t->u.xchg.src_bytes >= ((size_t)16 << 20)) t->use_ce = 1;
     *task_p = &t->super;
     return UCC_OK;
 }
