@@ -11,10 +11,6 @@
 
 #define NVL_LIB(_t) ((_t)->super.super.context->lib)
 
-/* kernels/nvl_swap.cu, linked into the plugin.  Weak, so that a plugin linked with a launcher set that lacks it (the host-emulated
- * plugin of tests/emu/build_hostemu.sh) still loads with immediate binding; such a plugin declines in-place alltoall(v) (xchg_init) */
-#pragma weak nvl_launch_exchange_swap
-
 static int to_nvl_dt(ucc_datatype_t dt)
 {
     switch (dt) {
@@ -829,7 +825,6 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     size_t moved = 0, dts;
     ucc_status_t st;
     if (team->self) return self_init(b, b_team, task_p);
-    if (inplace && (a->coll_type == UCC_COLL_TYPE_ALLTOALL || a->coll_type == UCC_COLL_TYPE_ALLTOALLV) && !nvl_launch_exchange_swap) return UCC_ERR_NOT_SUPPORTED;
     memset(&x, 0, sizeof(x));
     x.team = team->dev;
     if (UCC_COLL_ARGS_ACTIVE_SET(a)) {

@@ -2,10 +2,9 @@
 // complex data (one-shot, staged P2P and NVLS, zero-copy, ring, rhd, one-shot reduce_scatter(v), nvls_pipe, symmetric memory) at
 // every team-size class.  Inputs are Gaussian integers with components in {-2..2}: their sums and products over up to 8 ranks are
 // exact in float whatever the order, so SUM / PROD are compared bit for bit; AVG is exact for power-of-two teams.
+#include <cmath>
 #include <complex>
-#define main nvl_emu_main   // the World / launch_all harness of the real-type driver, without its main()
-#include "nvl_emu.cpp"
-#undef main
+#include "nvl_emu_world.h"
 
 template <typename R> static nvl_complex<R> cval(int r, size_t i)
 { return {(R)((int)((i * 7 + (size_t)r * 13) % 5) - 2), (R)((int)((i * 3 + (size_t)r * 11 + 1) % 5) - 2)}; }

@@ -2,10 +2,7 @@
 // (the pull kernel reading the peers' staged copies, run the way launch_swap in tl_nvl_coll.c runs it), team sizes 2, 3, 4 and 8.
 // Every case is checked here; given a directory, the driver also writes each result there for the NumPy oracle of
 // tests/test_nvl_swap.py.  Buffers start as init_byte(rank, offset) everywhere, gaps between the regions included.
-#define main nvl_emu_main   // the World / launch_all harness of the real-type driver, without its main()
-#include "nvl_emu.cpp"
-#undef main
-#include "nvl_swap.cu"
+#include "nvl_emu_world.h"
 
 static unsigned char init_byte(int r, size_t i)
 {

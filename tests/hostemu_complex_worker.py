@@ -1,5 +1,5 @@
 """Worker of tests/test_nvl_complex.py: complex float / double reductions through the public UCC API on the tl/nvl plugin built
-against the emulated CUDA runtime (tests/emu/build_hostemu_complex.sh), N ranks in this process.  Inputs are Gaussian integers with
+against the emulated CUDA runtime (tests/emu/build_hostemu.sh), N ranks in this process.  Inputs are Gaussian integers with
 components in {-2..2}, so SUM / PROD (and AVG on power-of-two teams) are exact and compared with equality."""
 import ctypes as C
 import os
@@ -8,19 +8,10 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from hostemu_worker import BASE, NOZC, ZC, Dev, U, UccJob, ca, coll_args, rt, run  # noqa: E402  (loads the emulated runtime)
-
-# the emulated plugin with the complex datatypes (tests/emu/build_hostemu_complex.sh), next to the runtime loaded above
-os.environ["UCC_MODULE_DIR"] = os.path.join(os.path.dirname(os.environ["UCC_MODULE_DIR"]), "ucc_complex")
+from hostemu_worker import BASE, NOZC, ZC, Dev, U, UccJob, ca, coll_args, last_launch, rt, run  # noqa: E402  (loads the emulated runtime)
 
 DTS = {"float32_complex": np.complex64, "float64_complex": np.complex128}
 TRACE = {"UCC_COLL_TRACE": "debug"}   # a coll_init line for every rank, naming the TL that serves the collective
-
-
-def last_launch():
-    info = C.CDLL(os.path.join(os.environ["UCC_MODULE_DIR"], "libucc_tl_nvl.so")).ucc_tl_nvl_last_launch_info
-    info.restype = C.c_char_p
-    return info().decode()
 
 
 def gauss(n, seed, dtype):

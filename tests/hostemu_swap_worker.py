@@ -1,5 +1,5 @@
 """Worker of tests/test_nvl_swap.py: in-place alltoall / alltoallv through the public UCC API on the tl/nvl plugin built against the
-emulated CUDA runtime with the swap kernel (tests/emu/build_hostemu_swap.sh), N ranks in this process.  Every result is compared with
+emulated CUDA runtime (tests/emu/build_hostemu.sh), N ranks in this process.  Every result is compared with
 numpy for equality; the launch note names the kernel that served it."""
 import ctypes as C
 import os
@@ -8,21 +8,10 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from hostemu_worker import BASE, NOZC, ZC, Dev, U, UccJob, ca, coll_args, rnd, rt, run  # noqa: E402  (loads the emulated runtime)
-
-# the emulated plugin with the swap kernel (tests/emu/build_hostemu_swap.sh), next to the runtime loaded above; scenario "no_swap_kernel"
-# keeps the plugin of tests/emu/build_hostemu.sh, whose launcher set lacks it
-if sys.argv[1:] != ["no_swap_kernel"]:
-    os.environ["UCC_MODULE_DIR"] = os.path.join(os.path.dirname(os.environ["UCC_MODULE_DIR"]), "ucc_swap")
+from hostemu_worker import BASE, NOZC, ZC, Dev, U, UccJob, ca, coll_args, last_launch, rnd, rt, run  # noqa: E402  (loads the emulated runtime)
 
 TRACE = {"UCC_COLL_TRACE": "debug"}   # a coll_init line for every rank, naming the TL that serves the collective
 SWAP, STAGED = "exchange_swap", "exchange_pull_staged_inplace"
-
-
-def last_launch():
-    info = C.CDLL(os.path.join(os.environ["UCC_MODULE_DIR"], "libucc_tl_nvl.so")).ucc_tl_nvl_last_launch_info
-    info.restype = C.c_char_p
-    return info().decode()
 
 
 def a2a_expect(bufs, n, blk):
@@ -202,25 +191,6 @@ def tune_swap():
     print("  TUNE alltoall:@swap ok", flush=True)
 
 
-def no_swap_kernel():
-    """a plugin linked without the swap launcher loads and declines in-place alltoall(v) at init: the request goes to the next TL
-    (test_nvl_swap.py checks the trace; it is only initialised here), out-of-place alltoall stays on tl/nvl"""
-    n, blk = 3, 1001
-    with UccJob(n, env=dict(BASE, **TRACE, **ZC)) as j:
-        team = j.create_team(range(n))
-        bufs = [Dev(blk * n, fill=rnd(blk * n, r)) for r in range(n)]
-        for r in range(n):
-            a = ca("alltoall", None, bufs[r], inplace=True)
-            q = C.POINTER(U.ucc_coll_req_t)()
-            assert U.ucc_collective_init(C.byref(a), C.byref(q), team.members[r].team) == U.UCC_OK
-            U.ucc_collective_finalize(q)
-        src = [Dev(blk * n, fill=rnd(blk * n, 10 + r)) for r in range(n)]
-        dst = [Dev(blk * n, fill=0) for _ in range(n)]
-        run(team, [ca("alltoall", src[r], dst[r]) for r in range(n)])
-        assert np.array_equal(dst[1].a, np.concatenate([s.a[blk:2 * blk] for s in src]))
-    print("  plugin without the swap kernel: in-place alltoall declined ok", flush=True)
-
-
 SCENARIOS = {
     "zcopy": lambda: inplace_colls(ZC, SWAP),
     "staged": lambda: inplace_colls(NOZC, STAGED),
@@ -228,7 +198,6 @@ SCENARIOS = {
     "memh": registered,
     "big_team": big_team,
     "tune": tune_swap,
-    "no_swap_kernel": no_swap_kernel,
 }
 
 if __name__ == "__main__":

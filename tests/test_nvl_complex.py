@@ -7,7 +7,7 @@ import sys
 
 import pytest
 
-from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin objects)
+from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA_INC = "/usr/local/cuda/include"
@@ -64,8 +64,6 @@ def test_complex_kernels_host_emulation(tmp_path):
 def test_complex_collectives_host_emulation(emu_build):  # noqa: F811
     """allreduce / reduce_scatter(v) / reduce on complex float and double, staged and zero-copy, in place and persistent: every rank's
     collective is served by tl/nvl, and a complex MAX never reaches it"""
-    b = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu_complex.sh")], capture_output=True, text=True, timeout=900)
-    assert "HOSTEMU_COMPLEX_BUILD_OK" in b.stdout, b.stdout[-2000:] + b.stderr[-3000:]
     env = dict(os.environ, PYTHONPATH=ROOT)
     for k in ("UCC_TL_NVL_TUNE", "UCC_MODULE_DIR", "UCC_TLS"):
         env.pop(k, None)

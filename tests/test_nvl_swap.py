@@ -9,7 +9,7 @@ import sys
 import numpy as np
 import pytest
 
-from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin objects)
+from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA_INC = "/usr/local/cuda/include"
@@ -67,14 +67,8 @@ def test_swap_kernels_host_emulation(tmp_path):
         assert (N, False, True, True, -1) in seen
 
 
-@pytest.fixture(scope="module")
-def swap_build(emu_build):  # noqa: F811
-    b = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu_swap.sh")], capture_output=True, text=True, timeout=900)
-    assert "HOSTEMU_SWAP_BUILD_OK" in b.stdout, b.stdout[-2000:] + b.stderr[-3000:]
-
-
 @pytest.mark.parametrize("scenario", ["zcopy", "staged", "persistent", "memh", "big_team", "tune"])
-def test_inplace_alltoall_host_emulation(swap_build, scenario):
+def test_inplace_alltoall_host_emulation(emu_build, scenario):  # noqa: F811
     """in-place alltoall / alltoallv through ucc_collective_init: every rank's request is served by tl/nvl, with the swap kernel
     or (UCC_TL_NVL_ZCOPY=n) the staged one"""
     env = dict(os.environ, PYTHONPATH=ROOT)
@@ -85,18 +79,3 @@ def test_inplace_alltoall_host_emulation(swap_build, scenario):
     inits = [ln for ln in (out.stdout + out.stderr).splitlines() if "coll_init: alltoall" in ln and " inplace" in ln]
     assert len(inits) >= 4, len(inits)
     assert all("{TL_NVL}" in ln for ln in inits), [ln for ln in inits if "{TL_NVL}" not in ln][:3]
-
-
-def test_plugin_without_swap_kernel(emu_build):  # noqa: F811
-    """the host-emulated plugin of tests/emu/build_hostemu.sh has no swap launcher: it still loads, and its in-place alltoall goes to the
-    next TL while out-of-place alltoall stays on tl/nvl"""
-    env = dict(os.environ, PYTHONPATH=ROOT)
-    for k in ("UCC_TL_NVL_TUNE", "UCC_MODULE_DIR", "UCC_TLS"):
-        env.pop(k, None)
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "hostemu_swap_worker.py"), "no_swap_kernel"], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0 and "HOSTEMU_WORKER_OK" in out.stdout, out.stdout[-2500:] + out.stderr[-2500:]
-    lines = (out.stdout + out.stderr).splitlines()
-    inplace = [ln for ln in lines if "coll_init: alltoall" in ln and " inplace" in ln]
-    other = [ln for ln in lines if "coll_init: alltoall" in ln and " inplace" not in ln]
-    assert len(inplace) == 3 and not any("{TL_NVL}" in ln for ln in inplace), inplace
-    assert len(other) == 3 and all("{TL_NVL}" in ln for ln in other), other
