@@ -229,8 +229,15 @@ template <> struct IsFloatLike<double> { static constexpr bool v = true; };
 template <> struct IsFloatLike<__half> { static constexpr bool v = true; };
 template <> struct IsFloatLike<__nv_bfloat16> { static constexpr bool v = true; };
 
-/* run F<T,OP>::run(args...) for the runtime operator; complex types have SUM / AVG / PROD only, bit/logic operators only exist
- * for integer types */
+/* the operators T has reduction kernels for, bit OP = operator OP: SUM / PROD / AVG for every type, MAX / MIN for the real ones,
+ * the logical and bitwise operators for integer types */
+template <typename T> struct OpsOf {
+    static constexpr uint32_t ARITH = 1u << NVL_OP_SUM | 1u << NVL_OP_PROD | 1u << NVL_OP_AVG, ORDER = 1u << NVL_OP_MAX | 1u << NVL_OP_MIN;
+    static constexpr uint32_t mask = IsComplex<T>::v ? ARITH : (IsFloatLike<T>::v ? ARITH | ORDER : (1u << NVL_OP_LAST) - 1);
+};
+
+/* _CALL(_T, OP) for the runtime operator _op if OpsOf<_T> has it, nothing otherwise; the switches follow the three groups of the
+ * mask */
 #define NVL_DISPATCH_OP(_T, _op, _CALL)                                                         \
     do {                                                                                        \
         switch (_op) {                                                                          \
@@ -238,12 +245,12 @@ template <> struct IsFloatLike<__nv_bfloat16> { static constexpr bool v = true; 
         case NVL_OP_AVG: _CALL(_T, NVL_OP_AVG); break;                                          \
         case NVL_OP_PROD: _CALL(_T, NVL_OP_PROD); break;                                        \
         default:                                                                                \
-            if constexpr (!IsComplex<_T>::v) {                                                  \
+            if constexpr ((OpsOf<_T>::mask >> NVL_OP_MAX) & 1) {                                \
                 switch (_op) {                                                                  \
                 case NVL_OP_MAX: _CALL(_T, NVL_OP_MAX); break;                                  \
                 case NVL_OP_MIN: _CALL(_T, NVL_OP_MIN); break;                                  \
                 default:                                                                        \
-                    if constexpr (!IsFloatLike<_T>::v) {                                        \
+                    if constexpr ((OpsOf<_T>::mask >> NVL_OP_LAND) & 1) {                       \
                         switch (_op) {                                                          \
                         case NVL_OP_LAND: _CALL(_T, NVL_OP_LAND); break;                        \
                         case NVL_OP_LOR: _CALL(_T, NVL_OP_LOR); break;                          \

@@ -212,73 +212,15 @@ __global__ void __launch_bounds__(NVL_THREADS_MAX, 2) nvl_exchange_kernel(nvl_xc
 /* host-side launchers                                                 */
 /* ------------------------------------------------------------------ */
 #ifndef NVL_HOST_EMU /* tests/emu includes the kernels above and calls them directly */
-extern "C" size_t nvl_dt_size(int dt)
+/* the rows of the reduction kernels in nvl_dt_t order, each defined by its nvl_red_<dt>.cu */
+extern const nvl_dt_row nvl_row_i8, nvl_row_i16, nvl_row_i32, nvl_row_i64, nvl_row_u8, nvl_row_u16, nvl_row_u32, nvl_row_u64, nvl_row_f16, nvl_row_f32,
+    nvl_row_f64, nvl_row_bf16, nvl_row_c64, nvl_row_c128;
+static const nvl_dt_row *const nvl_rows[NVL_DT_LAST] = {&nvl_row_i8, &nvl_row_i16, &nvl_row_i32, &nvl_row_i64, &nvl_row_u8, &nvl_row_u16, &nvl_row_u32,
+    &nvl_row_u64, &nvl_row_f16, &nvl_row_f32, &nvl_row_f64, &nvl_row_bf16, &nvl_row_c64, &nvl_row_c128};
+static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nblocks, int nthreads, cudaStream_t s)
 {
-    static const size_t s[NVL_DT_LAST] = {1, 2, 4, 8, 1, 2, 4, 8, 2, 4, 8, 2, 8, 16};
-    return dt >= 0 && dt < NVL_DT_LAST ? s[dt] : 0;
-}
-extern "C" int nvl_dt_supports_op(int dt, int op)
-{
-    if (dt < 0 || dt >= NVL_DT_LAST || op < 0 || op >= NVL_OP_LAST) return 0;
-    if (dt == NVL_DT_F16 || dt == NVL_DT_F32 || dt == NVL_DT_F64 || dt == NVL_DT_BF16)
-        return op == NVL_OP_SUM || op == NVL_OP_PROD || op == NVL_OP_MAX || op == NVL_OP_MIN || op == NVL_OP_AVG;
-    if (dt == NVL_DT_C64 || dt == NVL_DT_C128) return op == NVL_OP_SUM || op == NVL_OP_PROD || op == NVL_OP_AVG;
-    return 1;
-}
-extern "C" int nvl_nvls_supports(int dt, int op)
-{
-    /* mirrors the McRed<T,OP> specialisations: what multimem.ld_reduce can do for 16-byte vectors of that type */
-    if (dt == NVL_DT_F32 || dt == NVL_DT_BF16 || dt == NVL_DT_F16) return op == NVL_OP_SUM || op == NVL_OP_AVG;
-    if (dt == NVL_DT_C64) return op == NVL_OP_SUM || op == NVL_OP_AVG; /* the f32 vector add; no f64 / c128 in-switch path */
-    if (dt == NVL_DT_I32 || dt == NVL_DT_U32 || dt == NVL_DT_I64 || dt == NVL_DT_U64)
-        return op == NVL_OP_SUM || op == NVL_OP_MIN || op == NVL_OP_MAX || op == NVL_OP_BAND || op == NVL_OP_BOR || op == NVL_OP_BXOR;
-    return 0;
-}
-
-typedef cudaError_t (*nvl_red_launch_fn)(const nvl_red_args_t *, int, int, cudaStream_t);
-#define DECL(_s) extern "C" cudaError_t nvl_launch_oneshot_##_s(const nvl_red_args_t *, int, int, cudaStream_t); \
-                 extern "C" cudaError_t nvl_launch_staged_##_s(const nvl_red_args_t *, int, int, cudaStream_t);
-DECL(i8) DECL(i16) DECL(i32) DECL(i64) DECL(u8) DECL(u16) DECL(u32) DECL(u64) DECL(f16) DECL(f32) DECL(f64) DECL(bf16) DECL(c64) DECL(c128)
-static const nvl_red_launch_fn oneshot_fns[NVL_DT_LAST] = {nvl_launch_oneshot_i8, nvl_launch_oneshot_i16, nvl_launch_oneshot_i32, nvl_launch_oneshot_i64, nvl_launch_oneshot_u8, nvl_launch_oneshot_u16,
-    nvl_launch_oneshot_u32, nvl_launch_oneshot_u64, nvl_launch_oneshot_f16, nvl_launch_oneshot_f32, nvl_launch_oneshot_f64, nvl_launch_oneshot_bf16,
-    nvl_launch_oneshot_c64, nvl_launch_oneshot_c128};
-static const nvl_red_launch_fn staged_fns[NVL_DT_LAST] = {nvl_launch_staged_i8, nvl_launch_staged_i16, nvl_launch_staged_i32, nvl_launch_staged_i64, nvl_launch_staged_u8, nvl_launch_staged_u16,
-    nvl_launch_staged_u32, nvl_launch_staged_u64, nvl_launch_staged_f16, nvl_launch_staged_f32, nvl_launch_staged_f64, nvl_launch_staged_bf16,
-    nvl_launch_staged_c64, nvl_launch_staged_c128};
-
-extern "C" cudaError_t nvl_launch_allreduce_oneshot(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
-{
-    if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
-    if (a->dt < 0 || a->dt >= NVL_DT_LAST) return cudaErrorInvalidValue;
-    return oneshot_fns[a->dt](a, nblocks, nthreads, s);
-}
-extern "C" cudaError_t nvl_launch_reduce_staged(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
-{
-    if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
-    if (a->dt < 0 || a->dt >= NVL_DT_LAST) return cudaErrorInvalidValue;
-    return staged_fns[a->dt](a, nblocks, nthreads, s);
-}
-#define DECLD(_s) extern "C" cudaError_t nvl_launch_direct_##_s(const nvl_red_args_t *, int, int, cudaStream_t);
-DECLD(i8) DECLD(i16) DECLD(i32) DECLD(i64) DECLD(u8) DECLD(u16) DECLD(u32) DECLD(u64) DECLD(f16) DECLD(f32) DECLD(f64) DECLD(bf16) DECLD(c64) DECLD(c128)
-static const nvl_red_launch_fn direct_fns[NVL_DT_LAST] = {nvl_launch_direct_i8, nvl_launch_direct_i16, nvl_launch_direct_i32, nvl_launch_direct_i64, nvl_launch_direct_u8, nvl_launch_direct_u16,
-    nvl_launch_direct_u32, nvl_launch_direct_u64, nvl_launch_direct_f16, nvl_launch_direct_f32, nvl_launch_direct_f64, nvl_launch_direct_bf16,
-    nvl_launch_direct_c64, nvl_launch_direct_c128};
-extern "C" cudaError_t nvl_launch_reduce_direct(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
-{
-    if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
-    if (a->dt < 0 || a->dt >= NVL_DT_LAST) return cudaErrorInvalidValue;
-    return direct_fns[a->dt](a, nblocks, nthreads, s);
-}
-#define DECLS(_s) extern "C" cudaError_t nvl_launch_steps_##_s(const nvl_red_args_t *, int, int, cudaStream_t);
-DECLS(i8) DECLS(i16) DECLS(i32) DECLS(i64) DECLS(u8) DECLS(u16) DECLS(u32) DECLS(u64) DECLS(f16) DECLS(f32) DECLS(f64) DECLS(bf16) DECLS(c64) DECLS(c128)
-static const nvl_red_launch_fn steps_fns[NVL_DT_LAST] = {nvl_launch_steps_i8, nvl_launch_steps_i16, nvl_launch_steps_i32, nvl_launch_steps_i64, nvl_launch_steps_u8, nvl_launch_steps_u16,
-    nvl_launch_steps_u32, nvl_launch_steps_u64, nvl_launch_steps_f16, nvl_launch_steps_f32, nvl_launch_steps_f64, nvl_launch_steps_bf16,
-    nvl_launch_steps_c64, nvl_launch_steps_c128};
-extern "C" cudaError_t nvl_launch_reduce_steps(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
-{
-    if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
-    if (a->dt < 0 || a->dt >= NVL_DT_LAST) return cudaErrorInvalidValue;
-    return steps_fns[a->dt](a, nblocks, nthreads, s);
+    k<<<nblocks, nthreads, 0, s>>>(a);
+    return cudaGetLastError();
 }
 extern "C" cudaError_t nvl_launch_exchange(const nvl_xchg_args_t *a, int nblocks, int nthreads, cudaStream_t s)
 {
@@ -305,4 +247,36 @@ extern "C" cudaError_t nvl_launch_ctrl_init(void *heap_base, cudaStream_t s)
     nvl_ctrl_init_kernel<<<4, 256, 0, s>>>(static_cast<nvl_ctrl_t *>(heap_base));
     return cudaGetLastError();
 }
+#elif defined(NVL_EMU_LAUNCHERS)
+/* the host-emulated plugin (tests/emu/nvl_emu_launch.cpp) defines a table of the datatypes it builds and a run on its emulated
+ * stream */
+extern const nvl_dt_row *const nvl_rows[NVL_DT_LAST];
+static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nblocks, int nthreads, cudaStream_t s);
 #endif /* NVL_HOST_EMU */
+
+/* reductions: the datatype predicates and the launchers, the same in the GPU build and in the host-emulated plugin (the entry
+ * points of the one-shot reduce_scatter, nvls_pipe and symm kernels, which check more arguments, are in their own files) */
+#if !defined(NVL_HOST_EMU) || defined(NVL_EMU_LAUNCHERS)
+static const nvl_dt_row *nvl_row(int dt) { return dt >= 0 && dt < NVL_DT_LAST ? nvl_rows[dt] : nullptr; }
+extern "C" size_t nvl_dt_size(int dt) { const nvl_dt_row *r = nvl_row(dt); return r ? r->size : 0; }
+extern "C" int nvl_dt_supports_op(int dt, int op) { const nvl_dt_row *r = nvl_row(dt); return r && op >= 0 && op < NVL_OP_LAST && ((r->ops >> op) & 1); }
+extern "C" int nvl_nvls_supports(int dt, int op) { const nvl_dt_row *r = nvl_row(dt); return r && op >= 0 && op < NVL_OP_LAST && ((r->mc_ops >> op) & 1); }
+
+cudaError_t nvl_red_launch(int fam, const nvl_red_args_t *ap, int nblocks, int nthreads, cudaStream_t s)
+{
+    if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
+    const nvl_dt_row *r = nvl_row(ap->dt);
+    nvl_red_args_t a = *ap;
+    const nvl_red_kernel_t k = r ? r->select(fam, a) : nullptr;
+    if (!k) return cudaErrorInvalidValue;
+    return nvl_red_run(k, a, nblocks, nthreads, s);
+}
+extern "C" cudaError_t nvl_launch_allreduce_oneshot(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
+{ return nvl_red_launch(NVL_FAM_ONESHOT, a, nblocks, nthreads, s); }
+extern "C" cudaError_t nvl_launch_reduce_staged(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
+{ return nvl_red_launch(NVL_FAM_STAGED, a, nblocks, nthreads, s); }
+extern "C" cudaError_t nvl_launch_reduce_direct(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
+{ return nvl_red_launch(NVL_FAM_DIRECT, a, nblocks, nthreads, s); }
+extern "C" cudaError_t nvl_launch_reduce_steps(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
+{ return nvl_red_launch(NVL_FAM_STEPS, a, nblocks, nthreads, s); }
+#endif

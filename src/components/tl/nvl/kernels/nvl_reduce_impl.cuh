@@ -14,34 +14,9 @@
 
 /* Kernels are templates over (datatype, operator): the operator is chosen on the HOST at launch time, so each instantiation
  * carries exactly one reduction body (an operator switch inside the kernel made every kernel 11 bodies long and cost registers).
- *   GPU build : <name>_launch<T>(args, grid, block, stream) switches on args->op and launches <name>_t<T, OP>
- *   host emulation (tests/emu, kernels compiled as C++ functions): <name><T>(args) does the same switch and calls the body */
-#ifdef NVL_HOST_EMU
-#ifndef __grid_constant__
+ * nvl_select<T> at the end of this file picks the instantiation. */
+#if defined(NVL_HOST_EMU) && !defined(__grid_constant__)
 #define __grid_constant__
-#endif
-#define NVL_DEFINE_ENTRY(_name, _args_t)                                                                       \
-    template <typename T> static void _name(_args_t a)                                                          \
-    {                                                                                                          \
-        NVL_DISPATCH_OP(T, a.op, NVL_ENTRY_CALL_##_name);                                                      \
-    }
-#define NVL_ENTRY_CALL_nvl_allreduce_oneshot_kernel(_T, _OP) nvl_allreduce_oneshot_kernel_t<_T, _OP>(a)
-#define NVL_ENTRY_CALL_nvl_reduce_steps_kernel(_T, _OP) nvl_reduce_steps_kernel_t<_T, _OP>(a)
-#define NVL_ENTRY_CALL_nvl_allreduce_nvls_pipe_kernel(_T, _OP) nvl_allreduce_nvls_pipe_kernel_t<_T, _OP>(a)
-#define NVL_ENTRY_CALL_nvl_allreduce_symm_kernel(_T, _OP) nvl_allreduce_symm_kernel_t<_T, _OP>(a)
-#define NVL_ENTRY_CALL_nvl_reduce_scatter_oneshot_kernel(_T, _OP) nvl_reduce_scatter_oneshot_kernel_t<_T, _OP>(a)
-#else
-#define NVL_DEFINE_ENTRY(_name, _args_t)                                                                       \
-    template <typename T> static cudaError_t _name##_launch(const _args_t *ap, int nb, int nt, cudaStream_t s)  \
-    {                                                                                                          \
-        NVL_DISPATCH_OP(T, ap->op, NVL_ENTRY_CALL_##_name);                                                    \
-        return cudaGetLastError();                                                                             \
-    }
-#define NVL_ENTRY_CALL_nvl_allreduce_oneshot_kernel(_T, _OP) nvl_allreduce_oneshot_kernel_t<_T, _OP><<<nb, nt, 0, s>>>(*ap)
-#define NVL_ENTRY_CALL_nvl_reduce_steps_kernel(_T, _OP) nvl_reduce_steps_kernel_t<_T, _OP><<<nb, nt, 0, s>>>(*ap)
-#define NVL_ENTRY_CALL_nvl_allreduce_nvls_pipe_kernel(_T, _OP) nvl_allreduce_nvls_pipe_kernel_t<_T, _OP><<<nb, nt, 0, s>>>(*ap)
-#define NVL_ENTRY_CALL_nvl_allreduce_symm_kernel(_T, _OP) nvl_allreduce_symm_kernel_t<_T, _OP><<<nb, nt, 0, s>>>(*ap)
-#define NVL_ENTRY_CALL_nvl_reduce_scatter_oneshot_kernel(_T, _OP) nvl_reduce_scatter_oneshot_kernel_t<_T, _OP><<<nb, nt, 0, s>>>(*ap)
 #endif
 
 /* ------------------------------------------------------------------ */
@@ -135,14 +110,14 @@ template <typename T, int OP> __global__ void __launch_bounds__(NVL_THREADS_MAX)
     oneshot_body<T, OP>(a, mine, seq);
     ll_seq_end(mine, seq);
 }
-NVL_DEFINE_ENTRY(nvl_allreduce_oneshot_kernel, nvl_red_args_t)
 
 /* ------------------------------------------------------------------ */
 /* staged two-shot reduction: allreduce / reduce_scatter(v) / reduce   */
 /* ------------------------------------------------------------------ */
-/* (datatype, operator) pairs the NVSwitch can reduce; must mirror nvl_nvls_supports() in nvl_kernels.cu */
-template <typename T, int OP> struct McRed { static __device__ __forceinline__ uint4 ld(const void *) { return make_uint4(0, 0, 0, 0); } };
-#define NVL_MCRED(_T, _OP, _fn) template <> struct McRed<_T, _OP> { static __device__ __forceinline__ uint4 ld(const void *p) { return _fn(p); } };
+/* (datatype, operator) pairs the NVSwitch can reduce: only they have an ld, so an NVLS kernel of any other pair does not compile */
+template <typename T, int OP> struct McRed { static constexpr bool ok = false; };
+#define NVL_MCRED(_T, _OP, _fn) \
+    template <> struct McRed<_T, _OP> { static constexpr bool ok = true; static __device__ __forceinline__ uint4 ld(const void *p) { return _fn(p); } };
 NVL_MCRED(float, NVL_OP_SUM, mc_ld_reduce_f32) NVL_MCRED(float, NVL_OP_AVG, mc_ld_reduce_f32)
 /* complex float: re / im are interleaved floats, so the float vector sum is the complex sum */
 NVL_MCRED(nvl_c64, NVL_OP_SUM, mc_ld_reduce_f32) NVL_MCRED(nvl_c64, NVL_OP_AVG, mc_ld_reduce_f32)
@@ -156,6 +131,12 @@ NVL_MCRED(int64_t, NVL_OP_SUM, mc_red_add_u64) NVL_MCRED(int64_t, NVL_OP_MIN, mc
 NVL_MCRED(int64_t, NVL_OP_BAND, mc_red_and_b64) NVL_MCRED(int64_t, NVL_OP_BOR, mc_red_or_b64) NVL_MCRED(int64_t, NVL_OP_BXOR, mc_red_xor_b64)
 NVL_MCRED(uint64_t, NVL_OP_SUM, mc_red_add_u64) NVL_MCRED(uint64_t, NVL_OP_MIN, mc_red_min_u64) NVL_MCRED(uint64_t, NVL_OP_MAX, mc_red_max_u64)
 NVL_MCRED(uint64_t, NVL_OP_BAND, mc_red_and_b64) NVL_MCRED(uint64_t, NVL_OP_BOR, mc_red_or_b64) NVL_MCRED(uint64_t, NVL_OP_BXOR, mc_red_xor_b64)
+/* the same as a bit mask over the operators */
+template <typename T, int OP = 0> constexpr uint32_t mc_ops()
+{
+    if constexpr (OP == NVL_OP_LAST) return 0;
+    else return (McRed<T, OP>::ok ? 1u << OP : 0u) | mc_ops<T, OP + 1>();
+}
 
 /* Slice geometry.  Deliberately scalar: per-slice offsets / counts are recomputed from the kernel parameters (constant bank,
  * dynamically indexable) instead of living in a per-thread array, which the compiler would have to put on the local-memory stack. */
@@ -364,23 +345,6 @@ template <typename T, int OP, int MODE> __global__ void __launch_bounds__(NVL_BW
     staged_body<T, OP, MODE>(a, bs, pl);
     bs.finish(2 * (uint32_t)pl.rounds);
 }
-static inline int nvl_staged_mode(const nvl_red_args_t &a) { return (a.use_nvls && a.team.mc_heap) ? -1 : nvl_size_class(a.team.size); }
-#ifdef NVL_HOST_EMU
-#define NVL_STAGED_GO(_T, _OP, _M) nvl_reduce_staged_kernel_t<_T, _OP, _M>(a)
-#define NVL_STAGED_ARGS a
-#else
-#define NVL_STAGED_GO(_T, _OP, _M) nvl_reduce_staged_kernel_t<_T, _OP, _M><<<nb, nt, 0, s>>>(*ap)
-#define NVL_STAGED_ARGS (*ap)
-#endif
-#define NVL_CALL_STAGED(_T, _OP) do { switch (nvl_staged_mode(NVL_STAGED_ARGS)) { case -1: NVL_STAGED_GO(_T, _OP, -1); break; case 2: NVL_STAGED_GO(_T, _OP, 2); break; \
-    case 4: NVL_STAGED_GO(_T, _OP, 4); break; case 8: NVL_STAGED_GO(_T, _OP, 8); break; default: NVL_STAGED_GO(_T, _OP, 0); break; } } while (0)
-#ifdef NVL_HOST_EMU
-template <typename T> static void nvl_reduce_staged_kernel(nvl_red_args_t a) { NVL_DISPATCH_OP(T, a.op, NVL_CALL_STAGED); }
-#else
-template <typename T> static cudaError_t nvl_reduce_staged_kernel_launch(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s)
-{ NVL_DISPATCH_OP(T, ap->op, NVL_CALL_STAGED); return cudaGetLastError(); }
-#endif
-
 
 /* ------------------------------------------------------------------ */
 /* zero-copy two-shot: no staging, no copy-out                         */
@@ -446,47 +410,6 @@ template <typename T, int OP, int CN> __global__ void __launch_bounds__(NVL_BW_T
     bs.barrier(a.team, 2);
     bs.finish(2);
 }
-/* team-size class -> instantiation */
-template <typename T, int OP> struct nvl_reduce_direct_by_size {
-#ifdef NVL_HOST_EMU
-    static void run(const nvl_red_args_t &a)
-    {
-        switch (nvl_size_class(a.team.size)) {
-        case 2: nvl_reduce_direct_kernel_t<T, OP, 2>(a); break;
-        case 4: nvl_reduce_direct_kernel_t<T, OP, 4>(a); break;
-        case 8: nvl_reduce_direct_kernel_t<T, OP, 8>(a); break;
-        default: nvl_reduce_direct_kernel_t<T, OP, 0>(a); break;
-        }
-    }
-#else
-    static void launch(const nvl_red_args_t &a, int nb, int nt, cudaStream_t s)
-    {
-        switch (nvl_size_class(a.team.size)) {
-        case 2: nvl_reduce_direct_kernel_t<T, OP, 2><<<nb, nt, 0, s>>>(a); break;
-        case 4: nvl_reduce_direct_kernel_t<T, OP, 4><<<nb, nt, 0, s>>>(a); break;
-        case 8: nvl_reduce_direct_kernel_t<T, OP, 8><<<nb, nt, 0, s>>>(a); break;
-        default: nvl_reduce_direct_kernel_t<T, OP, 0><<<nb, nt, 0, s>>>(a); break;
-        }
-    }
-#endif
-};
-#ifdef NVL_HOST_EMU
-template <typename T> static void nvl_reduce_direct_kernel(nvl_red_args_t a)
-{
-    nvl_direct_rotate(&a);
-#define NVL_CALL_DIRECT(_T, _OP) nvl_reduce_direct_by_size<_T, _OP>::run(a)
-    NVL_DISPATCH_OP(T, a.op, NVL_CALL_DIRECT);
-}
-#else
-template <typename T> static cudaError_t nvl_reduce_direct_kernel_launch(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s)
-{
-    nvl_red_args_t a = *ap;
-    nvl_direct_rotate(&a);
-#define NVL_CALL_DIRECT(_T, _OP) nvl_reduce_direct_by_size<_T, _OP>::launch(a, nb, nt, s)
-    NVL_DISPATCH_OP(T, a.op, NVL_CALL_DIRECT);
-    return cudaGetLastError();
-}
-#endif
 
 /* ------------------------------------------------------------------ */
 /* step-structured allreduce / reduce_scatter through the heaps:       */
@@ -622,16 +545,77 @@ template <typename T, int OP> __global__ void __launch_bounds__(NVL_BW_THREADS, 
     steps_body<T, OP>(a, bs, pl, phase);
     bs.finish(phase);
 }
-NVL_DEFINE_ENTRY(nvl_reduce_steps_kernel, nvl_red_args_t)
 
-/* one translation unit per datatype defines these launchers */
-#define NVL_INSTANTIATE_REDUCE(_T, _suffix)                                                                              \
-    extern "C" cudaError_t nvl_launch_oneshot_##_suffix(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s) \
-    { return nvl_allreduce_oneshot_kernel_launch<_T>(a, nblocks, nthreads, s); }                                          \
-    extern "C" cudaError_t nvl_launch_staged_##_suffix(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)  \
-    { return nvl_reduce_staged_kernel_launch<_T>(a, nblocks, nthreads, s); }                                              \
-    extern "C" cudaError_t nvl_launch_direct_##_suffix(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)  \
-    { return nvl_reduce_direct_kernel_launch<_T>(a, nblocks, nthreads, s); }                                              \
-    extern "C" cudaError_t nvl_launch_steps_##_suffix(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)   \
-    { return nvl_reduce_steps_kernel_launch<_T>(a, nblocks, nthreads, s); }
+#include "nvl_oneshot_rs.cuh"
+#include "nvl_pipe.cuh"
+#include "nvl_symm.cuh"
+
+/* ------------------------------------------------------------------ */
+/* which instantiation runs                                            */
+/* ------------------------------------------------------------------ */
+/* a __global__ function on the GPU (launched with <<<>>>); in the host emulation the same function compiled as C++, called by
+ * every emulated thread */
+typedef void (*nvl_red_kernel_t)(nvl_red_args_t);
+enum { NVL_FAM_ONESHOT, NVL_FAM_ONESHOT_RS, NVL_FAM_STAGED, NVL_FAM_DIRECT, NVL_FAM_STEPS, NVL_FAM_PIPE, NVL_FAM_SYMM };
+
+/* the kernel of family fam for (T, OP) and the team-size class / NVLS mode of a; null when there is none (the NVLS kernels exist
+ * for the pairs the switch can reduce only).  The zero-copy kernel gets a's pointer tables rotated (nvl_direct_rotate). */
+template <typename T, int OP> static nvl_red_kernel_t nvl_select_op(int fam, nvl_red_args_t &a)
+{
+    constexpr bool mc = McRed<T, OP>::ok;
+    switch (fam) {
+    case NVL_FAM_ONESHOT: return nvl_allreduce_oneshot_kernel_t<T, OP>;
+    case NVL_FAM_ONESHOT_RS: return nvl_reduce_scatter_oneshot_kernel_t<T, OP>;
+    case NVL_FAM_STEPS: return nvl_reduce_steps_kernel_t<T, OP>;
+    case NVL_FAM_STAGED:
+        if (a.use_nvls && a.team.mc_heap) { if constexpr (mc) return nvl_reduce_staged_kernel_t<T, OP, -1>; else return nullptr; }
+        switch (nvl_size_class(a.team.size)) {
+        case 2: return nvl_reduce_staged_kernel_t<T, OP, 2>;
+        case 4: return nvl_reduce_staged_kernel_t<T, OP, 4>;
+        case 8: return nvl_reduce_staged_kernel_t<T, OP, 8>;
+        default: return nvl_reduce_staged_kernel_t<T, OP, 0>;
+        }
+    case NVL_FAM_DIRECT:
+        nvl_direct_rotate(&a);
+        switch (nvl_size_class(a.team.size)) {
+        case 2: return nvl_reduce_direct_kernel_t<T, OP, 2>;
+        case 4: return nvl_reduce_direct_kernel_t<T, OP, 4>;
+        case 8: return nvl_reduce_direct_kernel_t<T, OP, 8>;
+        default: return nvl_reduce_direct_kernel_t<T, OP, 0>;
+        }
+    case NVL_FAM_PIPE: if constexpr (mc) return nvl_allreduce_nvls_pipe_kernel_t<T, OP>; else return nullptr;
+    case NVL_FAM_SYMM: if constexpr (mc) return nvl_allreduce_symm_kernel_t<T, OP>; else return nullptr;
+    default: return nullptr;
+    }
+}
+/* ... for the operator a.op: null when T has no kernels for it */
+template <typename T> static nvl_red_kernel_t nvl_select(int fam, nvl_red_args_t &a)
+{
+#define NVL_SELECT_OP(_T, _OP) return nvl_select_op<_T, _OP>(fam, a)
+    NVL_DISPATCH_OP(T, a.op, NVL_SELECT_OP);
+    return nullptr;
+}
+/* the launcher of every reduction entry point (nvl_kernels.cu): thread clamp, datatype check, selection, launch */
+cudaError_t nvl_red_launch(int fam, const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s);
+
+#ifdef NVL_HOST_EMU
+/* host emulation (tests/emu): the kernel of a family for T and a.op, run by the calling emulated thread */
+template <typename T> static void nvl_emu_run(int fam, nvl_red_args_t a) { if (const nvl_red_kernel_t k = nvl_select<T>(fam, a)) k(a); }
+template <typename T> static void nvl_allreduce_oneshot_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_ONESHOT, a); }
+template <typename T> static void nvl_reduce_scatter_oneshot_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_ONESHOT_RS, a); }
+template <typename T> static void nvl_reduce_staged_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_STAGED, a); }
+template <typename T> static void nvl_reduce_direct_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_DIRECT, a); }
+template <typename T> static void nvl_reduce_steps_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_STEPS, a); }
+template <typename T> static void nvl_allreduce_nvls_pipe_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_PIPE, a); }
+template <typename T> static void nvl_allreduce_symm_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_SYMM, a); }
+#endif
+
+/* one datatype as the host sees it: nvl_red_<dt>.cu defines the row of its type, nvl_kernels.cu tables the rows by nvl_dt_t */
+struct nvl_dt_row {
+    size_t   size;
+    uint32_t ops, mc_ops;   /* bit OP: there are kernels for operator OP / the switch can reduce it */
+    nvl_red_kernel_t (*select)(int fam, nvl_red_args_t &a);
+};
+template <typename T> constexpr nvl_dt_row nvl_row_of = {sizeof(T), OpsOf<T>::mask, mc_ops<T>(), nvl_select<T>};
+#define NVL_INSTANTIATE_REDUCE(_T, _suffix) extern const nvl_dt_row nvl_row_##_suffix = nvl_row_of<_T>;
 #endif

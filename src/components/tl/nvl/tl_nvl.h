@@ -177,8 +177,8 @@ typedef struct ucc_tl_nvl_team {
 
 typedef enum { NVL_TASK_REDUCE_ONESHOT, NVL_TASK_REDUCE_STAGED, NVL_TASK_REDUCE_STEPS, NVL_TASK_XCHG, NVL_TASK_BARRIER,
                NVL_TASK_SELF_COPY /* team of one: u.xchg.{dst,src,src_bytes} describe the only data movement */,
-               NVL_TASK_REDUCE_PIPE /* pipelined staged NVLS allreduce (kernels/nvl_pipe.cu) */,
-               NVL_TASK_REDUCE_SYMM /* in-place NVLS allreduce on symmetric user memory (kernels/nvl_symm.cu) */,
+               NVL_TASK_REDUCE_PIPE /* pipelined staged NVLS allreduce (kernels/nvl_pipe.cuh) */,
+               NVL_TASK_REDUCE_SYMM /* in-place NVLS allreduce on symmetric user memory (kernels/nvl_symm.cuh) */,
                NVL_TASK_AG_SYMM /* allgather into a symmetric destination by multimem.st (u.xchg: src, src_bytes, dst, push_off) */,
                NVL_TASK_P2P /* two-member active-set bcast = send / recv over a heap channel (kernels/nvl_p2p.cu, u.p2p) */ } nvl_task_kind_t;
 typedef enum { NVL_TASK_LAUNCHED, NVL_TASK_QUEUED, NVL_TASK_P2P_WAIT /* send waiting for its turn / for the receiver's buffer */ } nvl_task_state_t;

@@ -706,7 +706,7 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
     if (ndt < 0 || nop < 0 || !nvl_dt_supports_op(ndt, nop)) return UCC_ERR_NOT_SUPPORTED;
     bytes = count * ucc_dt_size(dt);
     if (alg == RED_ALG_ONESHOT) {
-        /* allreduce: the whole vector goes into a 1 MB slot; reduce_scatter(v): every block does (kernels/nvl_oneshot_rs.cu) */
+        /* allreduce: the whole vector goes into a 1 MB slot; reduce_scatter(v): every block does (kernels/nvl_oneshot_rs.cuh) */
         size_t need = bytes;
         if (a->coll_type == UCC_COLL_TYPE_REDUCE_SCATTER) need = ucc_div_round_up(count, N) * ucc_dt_size(dt);
         else if (a->coll_type == UCC_COLL_TYPE_REDUCE_SCATTERV) { need = 0; for (ucc_rank_t i = 0; i < N; i++) need = ucc_max(need, ucc_coll_args_get_count(a, a->dst.info_v.counts, i) * ucc_dt_size(dt)); }
@@ -1181,7 +1181,7 @@ ucc_status_t ucc_tl_nvl_team_get_scores(ucc_base_team_t *b_team, ucc_coll_score_
      * reduction sends S (1 + 1/N) but adds two staging passes over HBM.  The gap grows with N (1.75 S against 1.125 S at
      * N = 8, 1.5 S against 1.25 S at N = 4), so NVLS is the default only for allreduce of at least ALLREDUCE_NVLS_THRESH
      * (512M) on teams of more than four, where the staging cost is spread over most bytes; `@nvls` remains selectable for
-     * everything.  The pipelined NVLS kernel (kernels/nvl_pipe.cu) overlaps stage / multimem / copy-out of consecutive rounds in
+     * everything.  The pipelined NVLS kernel (kernels/nvl_pipe.cuh) overlaps stage / multimem / copy-out of consecutive rounds in
      * three round buffers, hence the 384 MB default heap; it is chosen whenever the heap is big enough for them.  The size
      * thresholds were tuned on an earlier GPU generation and have not been measured on H100: retune them with
      * UCC_TL_NVL_TUNE on the box at hand */

@@ -1,5 +1,7 @@
 // Launchers of the tl/nvl kernels for the host-emulated build of the plugin: same C interface as kernels/nvl_kernels.h, but a
-// launch enqueues a closure on the emulated stream (cudart_emu.cpp) that runs the grid with one OS thread per CUDA thread.
+// launch enqueues a closure on the emulated stream (cudart_emu.cpp) that runs the grid with one OS thread per CUDA thread.  The
+// reduction entry points, their datatype predicates and the kernel selection are the kernel sources' own (NVL_EMU_LAUNCHERS).
+#define NVL_EMU_LAUNCHERS 1
 #include "nvl_emu_prelude.h"
 
 extern "C" void emu_stream_enqueue(cudaStream_t s, std::function<void()> *f);
@@ -25,41 +27,14 @@ template <typename F> static cudaError_t enqueue_grid(cudaStream_t s, int nb, in
     return cudaSuccess;
 }
 
-/* a representative subset of the datatypes keeps the build of this test-only plugin short */
-#define BY_DT(_a, _K)                                                                 \
-    switch ((_a).dt) {                                                                \
-    case NVL_DT_I32: return enqueue_grid(s, nb, nt, [a]() { _K<int32_t>(a); });       \
-    case NVL_DT_I64: return enqueue_grid(s, nb, nt, [a]() { _K<int64_t>(a); });       \
-    case NVL_DT_U8: return enqueue_grid(s, nb, nt, [a]() { _K<uint8_t>(a); });        \
-    case NVL_DT_F32: return enqueue_grid(s, nb, nt, [a]() { _K<float>(a); });         \
-    case NVL_DT_F64: return enqueue_grid(s, nb, nt, [a]() { _K<double>(a); });        \
-    case NVL_DT_BF16: return enqueue_grid(s, nb, nt, [a]() { _K<__nv_bfloat16>(a); }); \
-    case NVL_DT_C64: return enqueue_grid(s, nb, nt, [a]() { _K<nvl_c64>(a); });       \
-    case NVL_DT_C128: return enqueue_grid(s, nb, nt, [a]() { _K<nvl_c128>(a); });     \
-    default: return cudaErrorInvalidValue;                                            \
-    }
+static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nb, int nt, cudaStream_t s)
+{ return enqueue_grid(s, nb, nt, [k, a]() { k(a); }); }
 
-template <typename T> static void direct_any(nvl_red_args_t a) { nvl_reduce_direct_kernel<T>(a); }
+/* a representative subset of the datatypes keeps the build of this test-only plugin short; the others are not supported */
+const nvl_dt_row *const nvl_rows[NVL_DT_LAST] = {nullptr, nullptr, &nvl_row_of<int32_t>, &nvl_row_of<int64_t>, &nvl_row_of<uint8_t>, nullptr, nullptr,
+    nullptr, nullptr, &nvl_row_of<float>, &nvl_row_of<double>, &nvl_row_of<__nv_bfloat16>, &nvl_row_of<nvl_c64>, &nvl_row_of<nvl_c128>};
 
 extern "C" {
-size_t nvl_dt_size(int dt) { static const size_t sz[NVL_DT_LAST] = {1, 2, 4, 8, 1, 2, 4, 8, 2, 4, 8, 2, 8, 16}; return dt >= 0 && dt < NVL_DT_LAST ? sz[dt] : 0; }
-int nvl_dt_supports_op(int dt, int op)
-{
-    if (dt < 0 || dt >= NVL_DT_LAST || op < 0 || op >= NVL_OP_LAST) return 0;
-    if (dt != NVL_DT_I32 && dt != NVL_DT_I64 && dt != NVL_DT_U8 && dt != NVL_DT_F32 && dt != NVL_DT_F64 && dt != NVL_DT_BF16 && dt != NVL_DT_C64 && dt != NVL_DT_C128)
-        return 0; /* not built here: falls back to the next TL */
-    if (dt == NVL_DT_F16 || dt == NVL_DT_F32 || dt == NVL_DT_F64 || dt == NVL_DT_BF16) return op == NVL_OP_SUM || op == NVL_OP_PROD || op == NVL_OP_MAX || op == NVL_OP_MIN || op == NVL_OP_AVG;
-    if (dt == NVL_DT_C64 || dt == NVL_DT_C128) return op == NVL_OP_SUM || op == NVL_OP_PROD || op == NVL_OP_AVG;
-    return 1;
-}
-int nvl_nvls_supports(int, int) { return 0; }
-cudaError_t nvl_launch_allreduce_oneshot(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_red_args_t a = *ap; BY_DT(a, nvl_allreduce_oneshot_kernel) }
-cudaError_t nvl_launch_reduce_staged(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_red_args_t a = *ap; BY_DT(a, nvl_reduce_staged_kernel) }
-cudaError_t nvl_launch_reduce_direct(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_red_args_t a = *ap; BY_DT(a, direct_any) }
-cudaError_t nvl_launch_reduce_steps(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_red_args_t a = *ap; BY_DT(a, nvl_reduce_steps_kernel) }
-cudaError_t nvl_launch_reduce_scatter_oneshot(const nvl_red_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_red_args_t a = *ap; BY_DT(a, nvl_reduce_scatter_oneshot_kernel) }
-cudaError_t nvl_launch_reduce_pipe(const nvl_red_args_t *, int, int, cudaStream_t) { return cudaErrorInvalidValue; }   /* NVLS only */
-cudaError_t nvl_launch_reduce_symm(const nvl_red_args_t *, int, int, cudaStream_t) { return cudaErrorInvalidValue; }
 cudaError_t nvl_launch_allgather_symm(const nvl_xchg_args_t *, int, int, cudaStream_t) { return cudaErrorInvalidValue; }
 cudaError_t nvl_launch_exchange(const nvl_xchg_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_xchg_args_t a = *ap; return enqueue_grid(s, nb, nt, [a]() { nvl_exchange_kernel(a); }); }
 cudaError_t nvl_launch_exchange_push(const nvl_push_args_t *ap, int nb, int nt, cudaStream_t s) { nvl_push_args_t a = *ap; return enqueue_grid(s, nb, nt, [a]() { nvl_exchange_push_kernel(a); }); }

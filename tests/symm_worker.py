@@ -1,5 +1,5 @@
 """Worker for test_dist_gpu.py::test_multiproc_symm: allreduce on tensors inside the symmetric user region of the tl/nvl heap
-(in-place in-switch reduction, kernels/nvl_symm.cu).  Also prints the bus bandwidth of a large message next to the default path."""
+(in-place in-switch reduction, kernels/nvl_symm.cuh).  Also prints the bus bandwidth of a large message next to the default path."""
 import os
 import sys
 

@@ -114,7 +114,7 @@ def test_torch_backend_cuda():
 @pytest.mark.skipif(os.environ.get("UCC_B200_EXPERIMENTAL_TESTS") != "1", reason="opt-in multi-GPU test of nvls_pipe: set UCC_B200_EXPERIMENTAL_TESTS=1")
 @pytest.mark.parametrize("heap", ["128M", "24M"])
 def test_multiproc_nvls_pipe(heap):
-    """Pipelined staged NVLS allreduce (kernels/nvl_pipe.cu); the small heap forces many chunks so the three buffers rotate."""
+    """Pipelined staged NVLS allreduce (kernels/nvl_pipe.cuh); the small heap forces many chunks so the three buffers rotate."""
     n = min(2, torch.cuda.device_count()) if torch.cuda.is_available() else 0
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
@@ -123,7 +123,7 @@ def test_multiproc_nvls_pipe(heap):
 
 @pytest.mark.skipif(os.environ.get("UCC_B200_EXPERIMENTAL_TESTS") != "1", reason="opt-in multi-GPU test of the symmetric-memory allreduce: set UCC_B200_EXPERIMENTAL_TESTS=1")
 def test_multiproc_symm():
-    """allreduce on tensors inside the symmetric user region: in-place multimem.ld_reduce / multimem.st (kernels/nvl_symm.cu)"""
+    """allreduce on tensors inside the symmetric user region: in-place multimem.ld_reduce / multimem.st (kernels/nvl_symm.cuh)"""
     n = min(2, torch.cuda.device_count()) if torch.cuda.is_available() else 0
     if n < 2:
         pytest.skip("needs >= 2 GPUs")

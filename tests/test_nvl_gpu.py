@@ -196,7 +196,7 @@ def test_reduce_scatter(job, n, inplace):
 @pytest.mark.parametrize("n", [2, 3, 8])
 def test_reduce_scatter_oneshot_mixed_with_allreduce(n):
     """one-shot reduce_scatter(v) (push every block to its owner's latency slot, one flag exchange) interleaved with one-shot allreduces
-    of different grid sizes: both share the slot parity / team-wide sequence (kernels/nvl_oneshot_rs.cu)"""
+    of different grid sizes: both share the slot parity / team-wide sequence (kernels/nvl_oneshot_rs.cuh)"""
     need_cuda()
     env = dict(ENV, UCC_TL_NVL_TUNE="reduce_scatter:cuda:0-inf:@oneshot#reduce_scatterv:cuda:0-inf:@oneshot", **NOZC)
     with UccJob(n, env=env) as j:
