@@ -58,7 +58,6 @@ typedef struct ucc_tl_nvl_context_config {
 #define NVL_MAX_LANES 8
 #define NVL_EVENT_CACHE 256
 #define NVL_XB_SLOTS 64
-#define NVL_GATE_SLOTS 1024
 #define NVL_IPC_CACHE_MAX 64
 typedef enum { NVL_XB_NONE = 0, NVL_XB_EMPTY, NVL_XB_RAW, NVL_XB_IPC } nvl_xb_kind_t;
 typedef struct nvl_xb_buf { int32_t kind; int32_t pad; uint64_t base, off, len, alloc_len; cudaIpcMemHandle_t handle; } nvl_xb_buf_t;
@@ -138,7 +137,6 @@ typedef struct ucc_tl_nvl_team {
     nvl_team_dev_t    dev;
     cudaStream_t      stream;
     uint32_t         *host_err;             /* pinned, device mapped */
-    uint32_t          seq_num;
     /* zero-copy exchange */
     int               zcopy;                /* boards of all members are mapped */
     char              xb_name[48]; int xb_named;
@@ -171,21 +169,39 @@ typedef struct ucc_tl_nvl_team {
     uint32_t          rz_zc_tx[NVL_MAX_PEERS], rz_zc_rx[NVL_MAX_PEERS]; /* ... of those, the ones that really go zero-copy (device counter p2p_rz_done) */
     cudaStream_t      p2p_stream[NVL_MAX_PEERS];
     cudaEvent_t       p2p_side_event[NVL_MAX_PEERS]; int p2p_side_used[NVL_MAX_PEERS];
-    uint32_t         *gates;                /* device words user streams wait on while their collective is deferred */
-    uint32_t          gate_seq;
 } ucc_tl_nvl_team_t;
 
-typedef enum { NVL_TASK_REDUCE_ONESHOT, NVL_TASK_REDUCE_STAGED, NVL_TASK_REDUCE_STEPS, NVL_TASK_XCHG, NVL_TASK_BARRIER,
-               NVL_TASK_SELF_COPY /* team of one: u.xchg.{dst,src,src_bytes} describe the only data movement */,
-               NVL_TASK_REDUCE_PIPE /* pipelined staged NVLS allreduce (kernels/nvl_pipe.cuh) */,
-               NVL_TASK_REDUCE_SYMM /* in-place NVLS allreduce on symmetric user memory (kernels/nvl_symm.cuh) */,
-               NVL_TASK_AG_SYMM /* allgather into a symmetric destination by multimem.st (u.xchg: src, src_bytes, dst, push_off) */,
-               NVL_TASK_P2P /* two-member active-set bcast = send / recv over a heap channel (kernels/nvl_p2p.cu, u.p2p) */ } nvl_task_kind_t;
+/* How a task launches, chosen at init and never changed afterwards.  A post only resolves whether the members' buffers could be
+ * mapped (u.red.direct / u.xchg.direct): that bit picks the path's direct (zero-copy) form over its staged form, where it has one.
+ * Reduction paths use u.red, the ones from NVL_PATH_AG_SYMM to NVL_PATH_SELF_COPY_CE use u.xchg, send / recv uses u.p2p. */
+typedef enum {
+    NVL_PATH_ONESHOT,      /* one-shot allreduce */
+    NVL_PATH_ONESHOT_RS,   /* one-shot reduce_scatter(v) (kernels/nvl_oneshot_rs.cuh) */
+    NVL_PATH_TWOSHOT,      /* staged two-shot reduction; direct: in place in the members' buffers */
+    NVL_PATH_NVLS,         /* staged two-shot reduction through the switch */
+    NVL_PATH_RING,         /* step-structured reduction, ring schedule */
+    NVL_PATH_RHD,          /* step-structured reduction, recursive halving / doubling */
+    NVL_PATH_NVLS_PIPE,    /* pipelined staged NVLS allreduce (kernels/nvl_pipe.cuh) */
+    NVL_PATH_SYMM,         /* NVLS reduction on symmetric user memory, nothing staged (kernels/nvl_symm.cuh) */
+    NVL_PATH_AG_SYMM,      /* allgather into a symmetric destination by multimem.st (u.xchg: src, src_bytes, dst, push_off) */
+    NVL_PATH_PULL,         /* stage + pull exchange; direct: pull from the members' source buffers */
+    NVL_PATH_PULL_NVLS,    /* exchange whose staging multicasts into every heap (u.xchg.use_mc) */
+    NVL_PATH_PULL_RING,    /* allgather(v) in N-1 neighbour steps (u.xchg.ring) */
+    NVL_PATH_PUSH,         /* direct: store my blocks into the members' destinations (kernels/nvl_push.cu); staged: pull */
+    NVL_PATH_PUSH_BULK,    /* the same, moved by TMA bulk copies */
+    NVL_PATH_PUSH_CE,      /* the same, one cudaMemcpyAsync per peer between two barrier kernels */
+    NVL_PATH_SWAP,         /* in-place alltoall(v); direct: pairwise swap kernel (kernels/nvl_swap.cu); staged: self-copy + pull */
+    NVL_PATH_SELF_COPY,    /* team of one: u.xchg.{dst,src,src_bytes} describe the only data movement, copied by a kernel */
+    NVL_PATH_SELF_COPY_CE, /* ... copied by cudaMemcpyAsync */
+    NVL_PATH_BARRIER,
+    NVL_PATH_P2P,          /* two-member active-set bcast = send / recv over a heap channel (kernels/nvl_p2p.cu, u.p2p) */
+    NVL_PATH_NUM
+} nvl_path_t;
 typedef enum { NVL_TASK_LAUNCHED, NVL_TASK_QUEUED, NVL_TASK_P2P_WAIT /* send waiting for its turn / for the receiver's buffer */ } nvl_task_state_t;
 typedef struct ucc_tl_nvl_task {
     ucc_coll_task_t     super;
     ucc_tl_nvl_team_t  *team;
-    nvl_task_kind_t     kind;
+    nvl_path_t          path;
     union { nvl_red_args_t red; nvl_xchg_args_t xchg; nvl_p2p_args_t p2p; } u;
     int                 nblocks, nthreads;
     cudaEvent_t         event;
@@ -195,7 +211,7 @@ typedef struct ucc_tl_nvl_task {
     /* zero-copy / deferred launch */
     nvl_task_state_t    state;
     ucc_list_link_t     q_elem;
-    int                 want_direct;   /* try the in-place kernels for this collective (nvl_direct_mode_t, 0 = no) */
+    int                 want_direct;   /* try the path's direct form for this collective */
     int                 need_src, need_dst;
     const void         *exp_src; void *exp_dst; size_t exp_src_len, exp_dst_len; /* what is published to the peers */
     uint64_t            cseq;
@@ -204,10 +220,7 @@ typedef struct ucc_tl_nvl_task {
     int                 direct_cached; /* persistent request: the members' buffers were resolved by an earlier post (cached_mode / cached_d) */
     int                 cached_mode;
     nvl_direct_t        cached_d;
-    int                 gated;         /* the user's stream is parked on gates[gate_idx] until the deferred kernel ran */
-    uint32_t            gate_val;
     cudaEvent_t         in_event;
-    int                 nblocks_direct;
     /* send / recv */
     int                 p2p_rndv;      /* large message: rendezvous protocol */
     uint32_t            p2p_order;     /* send: position among the sends to this peer */
@@ -217,12 +230,7 @@ typedef struct ucc_tl_nvl_task {
     int                 rz_stream_idle;/* recv: the stream had nothing queued at post time */
     int                 rz_pub_pending;/* recv: the buffer is not on the board yet (stream not there yet / slot busy / not my turn) */
     nvl_xb_buf_t        rz_buf;        /* recv: what will be published */
-    /* zero-copy push exchange (kernels/nvl_push.cu): used instead of the pull kernel when the destinations resolved */
-    int                 use_bulk;      /* push exchange driven by the TMA engine (nvl_exchange_push_bulk_kernel) */
-    int                 use_ce;        /* push exchange executed by the copy engines (cudaMemcpyAsync between two barrier kernels); team of one: the copy is one cudaMemcpyAsync */
-    int                 use_push;
-    int                 use_swap;      /* in-place alltoall(v): pairwise swap kernel (kernels/nvl_swap.cu) when the buffers resolved,
-                                          else the heap-staged pull (nvl_launch) */
+    /* push paths: what the direct form stores where */
     struct { size_t send_off[NVL_MAX_PEERS], send_bytes[NVL_MAX_PEERS], land_off[NVL_MAX_PEERS], recv_off[NVL_MAX_PEERS], peer_land[NVL_MAX_PEERS]; int lookup; } push;
 } ucc_tl_nvl_task_t;
 

@@ -39,31 +39,51 @@ static inline int is_cuda(ucc_memory_type_t mt) { return mt == UCC_MEMORY_TYPE_C
 static cudaEvent_t event_get(ucc_tl_nvl_context_t *ctx);
 static char nvl_last_launch[128];
 UCC_EXPORT const char *ucc_tl_nvl_last_launch_info(void) { return nvl_last_launch; }
+/* launch notes of each path's staged and direct form.  threads / grid: what the note reports where that is not the task's nthreads /
+ * nblocks (grid -1: no grid) */
+typedef struct { const char *staged, *direct; int direct_threads, grid; } nvl_path_note_t;
+static const nvl_path_note_t nvl_path_notes[NVL_PATH_NUM] = {
+    [NVL_PATH_ONESHOT]      = {"oneshot"},
+    [NVL_PATH_ONESHOT_RS]   = {"oneshot_rs"},
+    [NVL_PATH_TWOSHOT]      = {"twoshot_staged", "twoshot_zcopy(direct)"},
+    [NVL_PATH_NVLS]         = {"nvls_staged"},
+    [NVL_PATH_RING]         = {"ring"},
+    [NVL_PATH_RHD]          = {"rhd"},
+    [NVL_PATH_NVLS_PIPE]    = {"nvls_pipe"},
+    [NVL_PATH_SYMM]         = {"nvls_symm_inplace"},
+    [NVL_PATH_AG_SYMM]      = {"allgather_symm_mc"},
+    [NVL_PATH_PULL]         = {"exchange_pull_staged", "exchange_pull_zcopy"},
+    [NVL_PATH_PULL_NVLS]    = {"exchange_nvls"},
+    [NVL_PATH_PULL_RING]    = {"exchange_ring"},
+    [NVL_PATH_PUSH]         = {"exchange_pull_staged", "exchange_push"},
+    [NVL_PATH_PUSH_BULK]    = {"exchange_pull_staged", "exchange_push_bulk(tma)", 32},
+    [NVL_PATH_PUSH_CE]      = {"exchange_pull_staged", "exchange_push_copy_engine"},
+    [NVL_PATH_SWAP]         = {"exchange_pull_staged_inplace", "exchange_swap"},
+    [NVL_PATH_SELF_COPY]    = {"self_copy"},
+    [NVL_PATH_SELF_COPY_CE] = {"self_copy(cudaMemcpyAsync)", NULL, 0, -1},
+    [NVL_PATH_BARRIER]      = {"barrier", NULL, 0, 1},
+};
+static inline int path_uses_xchg(nvl_path_t p) { return p >= NVL_PATH_AG_SYMM && p <= NVL_PATH_SELF_COPY_CE; }
+static inline int path_is_push(nvl_path_t p) { return p == NVL_PATH_PUSH || p == NVL_PATH_PUSH_BULK || p == NVL_PATH_PUSH_CE; }
+/* this post runs the direct form of its path: the members' buffers resolved */
+static inline int task_runs_direct(const ucc_tl_nvl_task_t *t)
+{ return path_uses_xchg(t->path) ? t->u.xchg.direct : t->u.red.direct != NVL_DIRECT_NONE; }
+
 static void note_launch(const ucc_tl_nvl_task_t *t)
 {
-    const char *k = "barrier"; int nb = t->nblocks;
-    switch (t->kind) {
-    case NVL_TASK_REDUCE_ONESHOT: k = t->u.red.kind == NVL_RED_REDUCE_SCATTER ? "oneshot_rs" : "oneshot"; break;
-    case NVL_TASK_REDUCE_STAGED:
-        if (t->u.red.direct == NVL_DIRECT_FULL) { k = "twoshot_zcopy(direct)"; nb = t->nblocks_direct; }
-        else k = (t->u.red.use_nvls && t->team->nvls) ? "nvls_staged" : "twoshot_staged";
-        break;
-    case NVL_TASK_REDUCE_STEPS: k = t->u.red.sched == 1 ? "ring" : "rhd"; break;
-    case NVL_TASK_REDUCE_PIPE: k = "nvls_pipe"; break;
-    case NVL_TASK_REDUCE_SYMM: k = "nvls_symm_inplace"; break;
-    case NVL_TASK_AG_SYMM: k = "allgather_symm_mc"; break;
-    case NVL_TASK_XCHG: k = t->use_swap ? (t->u.xchg.direct ? "exchange_swap" : "exchange_pull_staged_inplace") : (t->use_push && t->u.xchg.direct) ? (t->use_ce ? "exchange_push_copy_engine" : (t->use_bulk ? "exchange_push_bulk(tma)" : "exchange_push")) : (t->u.xchg.direct ? "exchange_pull_zcopy" : (t->u.xchg.use_mc ? "exchange_nvls" : (t->u.xchg.ring ? "exchange_ring" : "exchange_pull_staged"))); break;
-    case NVL_TASK_SELF_COPY:
-        if (t->use_ce) { snprintf(nvl_last_launch, sizeof(nvl_last_launch), "self_copy(cudaMemcpyAsync)"); return; }   /* no grid */
-        k = "self_copy"; break;
-    case NVL_TASK_P2P:
+    const nvl_path_note_t *n = &nvl_path_notes[t->path];
+    const char *k; int nb, direct;
+    if (t->path == NVL_PATH_P2P) { /* named by the rendezvous mode of this post */
         if (t->u.p2p.mode == NVL_P2P_PUSH) { k = "p2p_send_rndv(push)"; nb = nvl_p2p_push_ctas(t->u.p2p.bytes); }
         else if (t->u.p2p.mode == NVL_P2P_WAIT) { k = "p2p_recv_rndv(wait)"; nb = 1; }
         else { k = t->u.p2p.send ? "p2p_send" : "p2p_recv"; nb = nvl_p2p_lanes(t->u.p2p.bytes); }
-        break;
-    default: nb = 1; break;
+        snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", k, nb, t->nthreads);
+        return;
     }
-    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", k, nb, (t->use_bulk && !t->use_ce && t->use_push && t->u.xchg.direct) ? 32 : t->nthreads);
+    if (n->grid < 0) { snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s", n->staged); return; }
+    direct = task_runs_direct(t);
+    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", direct ? n->direct : n->staged, n->grid ? n->grid : t->nblocks,
+             direct && n->direct_threads ? n->direct_threads : t->nthreads);
 }
 
 /* in-place alltoall(v).  Buffers resolved: one swap kernel trades every pair of regions between the mapped buffers.  Otherwise my
@@ -91,60 +111,61 @@ static cudaError_t launch_swap(ucc_tl_nvl_task_t *t, cudaStream_t s)
     return nvl_launch_exchange(&x, t->nblocks, t->nthreads, s);
 }
 
+/* every member's destination resolved: store my blocks straight into them */
+static cudaError_t launch_push(ucc_tl_nvl_task_t *t, cudaStream_t s)
+{
+    nvl_push_args_t pa;
+    cudaError_t e;
+    memset(&pa, 0, sizeof(pa));
+    pa.team = t->u.xchg.team; pa.src = t->u.xchg.src;
+    for (int p = 0; p < pa.team.size; p++) {
+        pa.send_off[p] = t->push.send_off[p]; pa.send_bytes[p] = t->push.send_bytes[p]; pa.land_off[p] = t->push.land_off[p]; pa.recv_off[p] = t->push.recv_off[p];
+        pa.dst_of[p] = p == pa.team.rank ? (char *)t->u.xchg.dst : t->u.xchg.d.dst[p];
+    }
+    pa.lookup = t->push.lookup;
+    if (t->path == NVL_PATH_PUSH_BULK) return nvl_launch_exchange_push_bulk(&pa, t->nblocks, s);
+    if (t->path == NVL_PATH_PUSH) return nvl_launch_exchange_push(&pa, t->nblocks, t->nthreads, s);
+    /* copy-engine variant (reference tl/cuda alltoallv_ce.c:202-439: cudaMemcpyAsync per peer after an IPC handle exchange and a
+     * host barrier): barrier kernel (every member's stream reached the collective: its dst may be written) -> one DMA per peer,
+     * straight into the mapped destinations; no SM moves a byte -> barrier kernel (everything has landed).  The landing offsets
+     * of alltoallv travelled with the buffer exchange (peer_land). */
+    e = nvl_launch_barrier(&t->u.xchg.team, s);
+    for (int i = 1; i <= pa.team.size && e == cudaSuccess; i++) {
+        int p = (pa.team.rank + i) % pa.team.size;
+        size_t land = pa.lookup ? t->push.peer_land[p] : pa.land_off[p];
+        if (!pa.send_bytes[p] || pa.dst_of[p] + land == (const char *)pa.src + pa.send_off[p]) continue;
+        e = cudaMemcpyAsync(pa.dst_of[p] + land, (const char *)pa.src + pa.send_off[p], pa.send_bytes[p], cudaMemcpyDeviceToDevice, s);
+    }
+    if (e == cudaSuccess) e = nvl_launch_barrier(&t->u.xchg.team, s);
+    return e;
+}
+
 static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
 {
+    const nvl_xchg_args_t *x = &t->u.xchg;
     cudaError_t e;
     note_launch(t);
-    switch (t->kind) {
-    case NVL_TASK_REDUCE_ONESHOT:
-        e = t->u.red.kind == NVL_RED_REDUCE_SCATTER ? nvl_launch_reduce_scatter_oneshot(&t->u.red, t->nblocks, t->nthreads, s)
-                                                    : nvl_launch_allreduce_oneshot(&t->u.red, t->nblocks, t->nthreads, s);
-        break;
-    case NVL_TASK_REDUCE_STAGED:
-        if (t->u.red.direct == NVL_DIRECT_FULL) e = nvl_launch_reduce_direct(&t->u.red, t->nblocks_direct, t->nthreads, s);
-        else e = nvl_launch_reduce_staged(&t->u.red, t->nblocks, t->nthreads, s);
-        break;
-    case NVL_TASK_REDUCE_STEPS: e = nvl_launch_reduce_steps(&t->u.red, t->nblocks, t->nthreads, s); break;
-    case NVL_TASK_REDUCE_PIPE: e = nvl_launch_reduce_pipe(&t->u.red, t->nblocks, t->nthreads, s); break;
-    case NVL_TASK_REDUCE_SYMM: e = nvl_launch_reduce_symm(&t->u.red, t->nblocks, t->nthreads, s); break;
-    case NVL_TASK_AG_SYMM: e = nvl_launch_allgather_symm(&t->u.xchg, t->nblocks, t->nthreads, s); break;
-    case NVL_TASK_XCHG:
-        if (t->use_swap) e = launch_swap(t, s);
-        else if (t->use_push && t->u.xchg.direct) { /* every member's destination resolved: store my blocks straight into them */
-            nvl_push_args_t pa;
-            memset(&pa, 0, sizeof(pa));
-            pa.team = t->u.xchg.team; pa.src = t->u.xchg.src;
-            for (int p = 0; p < pa.team.size; p++) {
-                pa.send_off[p] = t->push.send_off[p]; pa.send_bytes[p] = t->push.send_bytes[p]; pa.land_off[p] = t->push.land_off[p]; pa.recv_off[p] = t->push.recv_off[p];
-                pa.dst_of[p] = p == pa.team.rank ? (char *)t->u.xchg.dst : t->u.xchg.d.dst[p];
-            }
-            pa.lookup = t->push.lookup;
-            /* (every member takes this branch or none: `direct` is decided from what all of them published) */
-            if (t->use_ce) {
-                /* copy-engine variant (reference tl/cuda alltoallv_ce.c:202-439: cudaMemcpyAsync per peer after an IPC handle
-                 * exchange and a host barrier): barrier kernel (every member's stream reached the collective: its dst may be
-                 * written) -> one DMA per peer, straight into the mapped destinations; no SM moves a byte -> barrier kernel
-                 * (everything has landed).  The landing offsets of alltoallv travelled with the buffer exchange (peer_land). */
-                e = nvl_launch_barrier(&t->u.xchg.team, s);
-                for (int i = 1; i <= pa.team.size && e == cudaSuccess; i++) {
-                    int p = (pa.team.rank + i) % pa.team.size;
-                    size_t land = pa.lookup ? t->push.peer_land[p] : pa.land_off[p];
-                    if (!pa.send_bytes[p] || pa.dst_of[p] + land == (const char *)pa.src + pa.send_off[p]) continue;
-                    e = cudaMemcpyAsync(pa.dst_of[p] + land, (const char *)pa.src + pa.send_off[p], pa.send_bytes[p], cudaMemcpyDeviceToDevice, s);
-                }
-                if (e == cudaSuccess) e = nvl_launch_barrier(&t->u.xchg.team, s);
-                break;
-            }
-            e = t->use_bulk ? nvl_launch_exchange_push_bulk(&pa, t->nblocks, s) : nvl_launch_exchange_push(&pa, t->nblocks, t->nthreads, s);
-        } else e = nvl_launch_exchange(&t->u.xchg, t->nblocks, t->nthreads, s);
-        break;
-    case NVL_TASK_P2P: e = nvl_launch_p2p(&t->u.p2p, t->nthreads, s); break;
-    case NVL_TASK_SELF_COPY:
-        if (!t->u.xchg.src_bytes) e = cudaSuccess;
-        else if (t->use_ce) e = cudaMemcpyAsync(t->u.xchg.dst, t->u.xchg.src, t->u.xchg.src_bytes, cudaMemcpyDeviceToDevice, s);
-        else e = nvl_launch_self_copy(t->u.xchg.dst, t->u.xchg.src, t->u.xchg.src_bytes, t->nblocks, t->nthreads, s);
-        break;
-    default: e = nvl_launch_barrier(&t->u.red.team, s); break;
+    switch (t->path) {
+    case NVL_PATH_ONESHOT: e = nvl_launch_allreduce_oneshot(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_ONESHOT_RS: e = nvl_launch_reduce_scatter_oneshot(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_TWOSHOT:
+        if (task_runs_direct(t)) { e = nvl_launch_reduce_direct(&t->u.red, t->nblocks, t->nthreads, s); break; }
+        /* fall through */
+    case NVL_PATH_NVLS: e = nvl_launch_reduce_staged(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_RING: case NVL_PATH_RHD: e = nvl_launch_reduce_steps(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_NVLS_PIPE: e = nvl_launch_reduce_pipe(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_SYMM: e = nvl_launch_reduce_symm(&t->u.red, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_AG_SYMM: e = nvl_launch_allgather_symm(x, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_PUSH: case NVL_PATH_PUSH_BULK: case NVL_PATH_PUSH_CE:
+        /* (every member takes the direct form or none: `direct` is decided from what all of them published) */
+        if (task_runs_direct(t)) { e = launch_push(t, s); break; }
+        /* fall through */
+    case NVL_PATH_PULL: case NVL_PATH_PULL_NVLS: case NVL_PATH_PULL_RING: e = nvl_launch_exchange(x, t->nblocks, t->nthreads, s); break;
+    case NVL_PATH_SWAP: e = launch_swap(t, s); break;
+    case NVL_PATH_SELF_COPY: e = x->src_bytes ? nvl_launch_self_copy(x->dst, x->src, x->src_bytes, t->nblocks, t->nthreads, s) : cudaSuccess; break;
+    case NVL_PATH_SELF_COPY_CE: e = x->src_bytes ? cudaMemcpyAsync(x->dst, x->src, x->src_bytes, cudaMemcpyDeviceToDevice, s) : cudaSuccess; break;
+    case NVL_PATH_P2P: e = nvl_launch_p2p(&t->u.p2p, t->nthreads, s); break;
+    case NVL_PATH_BARRIER: default: e = nvl_launch_barrier(&t->u.red.team, s); break;
     }
     if (e != cudaSuccess) { tl_error(NVL_LIB(t->team), "kernel launch failed: %s", cudaGetErrorString(e)); return UCC_ERR_NO_MESSAGE; }
     return UCC_OK;
@@ -157,12 +178,6 @@ static ucc_status_t launch_ordered(ucc_tl_nvl_task_t *t, cudaStream_t s)
     ucc_tl_nvl_team_t *team = t->team;
     ucc_status_t st;
     if (t->captured) return nvl_launch(t, s);
-    if (t->kind == NVL_TASK_P2P) { /* channel counters, no barrier epochs: independent of the team's collective order */
-        st = nvl_launch(t, s);
-        if (st != UCC_OK) return st;
-        CUDA_CHECK(cudaEventRecord(t->event, s));
-        return UCC_OK;
-    }
     if (team->last_event[t->lane] && team->last_stream[t->lane] != s) CUDA_CHECK(cudaStreamWaitEvent(s, team->last_event[t->lane], 0));
     st = nvl_launch(t, s);
     if (st != UCC_OK) return st;
@@ -176,10 +191,9 @@ static ucc_status_t launch_ordered(ucc_tl_nvl_task_t *t, cudaStream_t s)
 static void task_set_lane(ucc_tl_nvl_task_t *t, unsigned lane)
 {
     ucc_tl_nvl_team_t *team = t->team;
-    nvl_team_dev_t *d = (t->kind == NVL_TASK_XCHG || t->kind == NVL_TASK_AG_SYMM) ? &t->u.xchg.team : &t->u.red.team;
+    nvl_team_dev_t *d = path_uses_xchg(t->path) ? &t->u.xchg.team : &t->u.red.team;
     size_t off = (size_t)lane * team->lane_stride;
     t->lane = lane;
-    if (t->kind == NVL_TASK_SELF_COPY || t->kind == NVL_TASK_P2P) return;
     for (int p = 0; p < team->dev.size; p++) d->heap[p] = team->dev.heap[p] + off;
     d->mc_heap = team->dev.mc_heap ? team->dev.mc_heap + off : NULL;
 }
@@ -189,15 +203,15 @@ static void task_set_lane(ucc_tl_nvl_task_t *t, unsigned lane)
 static ucc_status_t resolve_direct(ucc_tl_nvl_task_t *t)
 {
     nvl_direct_t d;
-    int ok = ucc_tl_nvl_xb_resolve(t->team, t->cseq, t->need_src, t->need_dst, t->kind != NVL_TASK_XCHG, t->exp_src, t->exp_dst, &d, (t->kind == NVL_TASK_XCHG && t->use_push) ? t->push.peer_land : NULL);
+    int ok = ucc_tl_nvl_xb_resolve(t->team, t->cseq, t->need_src, t->need_dst, !path_uses_xchg(t->path), t->exp_src, t->exp_dst, &d, path_is_push(t->path) ? t->push.peer_land : NULL);
     tl_debug(NVL_LIB(t->team), "exchange %lu: %s (src %d dst %d)", (unsigned long)t->cseq, ok > 0 ? "zero-copy" : (ok ? "MAPPING FAILED" : "staged"), t->need_src, t->need_dst);
     if (ok < 0) {
         tl_error(NVL_LIB(t->team), "cannot map a peer's buffer for the zero-copy kernel (the peers will run it): failing the collective; "
                  "UCC_TL_NVL_ZCOPY=n avoids the zero-copy path");
         return UCC_ERR_NO_RESOURCE;
     }
-    if (t->kind == NVL_TASK_XCHG) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = d; }
-    else { t->u.red.direct = ok ? t->want_direct : NVL_DIRECT_NONE; if (ok) t->u.red.d = d; }
+    if (path_uses_xchg(t->path)) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = d; }
+    else { t->u.red.direct = ok ? NVL_DIRECT_FULL : NVL_DIRECT_NONE; if (ok) t->u.red.d = d; }
     /* persistent request: the buffers are fixed for the lifetime of the request, so every later post of it (same decision on
      * every member - they all re-post the same request) launches straight away with these tables: no handle export, no board
      * round trip, no deferred launch */
@@ -207,8 +221,8 @@ static ucc_status_t resolve_direct(ucc_tl_nvl_task_t *t)
 static void apply_cached_direct(ucc_tl_nvl_task_t *t)
 {
     int ok = t->cached_mode;
-    if (t->kind == NVL_TASK_XCHG) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = t->cached_d; }
-    else { t->u.red.direct = ok ? t->want_direct : NVL_DIRECT_NONE; if (ok) t->u.red.d = t->cached_d; }
+    if (path_uses_xchg(t->path)) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = t->cached_d; }
+    else { t->u.red.direct = ok ? NVL_DIRECT_FULL : NVL_DIRECT_NONE; if (ok) t->u.red.d = t->cached_d; }
 }
 static inline int task_is_direct(const ucc_tl_nvl_task_t *t) { return t->want_direct && (t->team->zcopy || t->direct_cached); }
 
@@ -395,7 +409,7 @@ static ucc_status_t try_launch_queued(ucc_tl_nvl_task_t *t)
     ucc_status_t st;
     if (ucc_list_head(&team->launch_q, ucc_tl_nvl_task_t, q_elem) != t) return UCC_INPROGRESS;
     if (t->need_xchg) {
-        if (!t->published) t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, 1, (t->kind == NVL_TASK_XCHG && t->use_push) ? t->push.recv_off : NULL);
+        if (!t->published) t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, 1, path_is_push(t->path) ? t->push.recv_off : NULL);
         if (!t->published || !ucc_tl_nvl_xb_ready(team, t->cseq)) return UCC_INPROGRESS;
         st = resolve_direct(t);
         if (st != UCC_OK) { ucc_list_del(&t->q_elem); t->state = NVL_TASK_LAUNCHED; return st; }
@@ -416,7 +430,7 @@ static void nvl_progress(ucc_coll_task_t *ct)
 {
     ucc_tl_nvl_task_t *t = ucc_derived_of(ct, ucc_tl_nvl_task_t);
     cudaError_t e;
-    if (t->kind == NVL_TASK_P2P && (t->rz_pub_pending || t->rz_wait_pending || t->state == NVL_TASK_P2P_WAIT)) {
+    if (t->path == NVL_PATH_P2P && (t->rz_pub_pending || t->rz_wait_pending || t->state == NVL_TASK_P2P_WAIT)) {
         ucc_status_t st = UCC_OK;
         ucc_spin_lock(&t->team->launch_lock);
         p2p_try_publish(t);
@@ -438,7 +452,7 @@ static void nvl_progress(ucc_coll_task_t *ct)
             ucc_ee_set_event_internal(t->super.ee, &post_event, &t->super.ee->event_out_queue);
         }
     }
-    if (t->kind == NVL_TASK_P2P && t->rz_wait_pending) return;   /* its event is not recorded yet */
+    if (t->path == NVL_PATH_P2P && t->rz_wait_pending) return;   /* its event is not recorded yet */
     if (t->state == NVL_TASK_QUEUED) {
         ucc_status_t st;
         ucc_spin_lock(&t->team->launch_lock);
@@ -485,31 +499,31 @@ static ucc_status_t nvl_post_on(ucc_tl_nvl_task_t *t, cudaStream_t s)
     ucc_tl_nvl_team_t *team = t->team;
     int direct;
     if (ucc_unlikely(t->super.flags & UCC_COLL_TASK_FLAG_ARGS_UPDATED)) { st = nvl_rebuild(t); if (st != UCC_OK) return st; }
-    t->stream = s; t->captured = 0; t->state = NVL_TASK_LAUNCHED; t->gated = 0; t->published = 0;
+    t->stream = s; t->captured = 0; t->state = NVL_TASK_LAUNCHED; t->published = 0;
     if (cudaStreamIsCapturing(s, &cs) == cudaSuccess && cs == cudaStreamCaptureStatusActive) t->captured = 1;
     ucc_spin_lock(&team->launch_lock);
     /* lanes advance in post order, which UCC requires to be the same on every member; point-to-point and single-member tasks
      * involve no team-wide kernel and take no lane */
-    if (t->kind == NVL_TASK_P2P) {
+    if (t->path == NVL_PATH_P2P) {
         t->p2p_ee_done = 0;
         st = p2p_post(t, s);
         ucc_spin_unlock(&team->launch_lock);
         if (st != UCC_OK) return st;
         return ucc_progress_queue_enqueue(UCC_TL_CORE_CTX(t->team)->pq, &t->super);
     }
-    if (t->kind != NVL_TASK_SELF_COPY) task_set_lane(t, team->lane_seq++ % team->nlanes);
+    if (t->path != NVL_PATH_SELF_COPY && t->path != NVL_PATH_SELF_COPY_CE) task_set_lane(t, team->lane_seq++ % team->nlanes);
     direct = task_is_direct(t) && !t->direct_cached;   /* cached tables: also fine inside a stream capture, nothing to wait for */
     t->need_xchg = direct;
-    if (t->kind == NVL_TASK_XCHG || t->kind == NVL_TASK_AG_SYMM) t->u.xchg.direct = 0; else if (t->kind != NVL_TASK_P2P) t->u.red.direct = NVL_DIRECT_NONE;
+    if (path_uses_xchg(t->path)) t->u.xchg.direct = 0; else t->u.red.direct = NVL_DIRECT_NONE;
     if (task_is_direct(t) && t->direct_cached) apply_cached_direct(t);
     if (direct) {
         /* the exchange sequence advances on every rank in post order; a capturing stream cannot wait for the
          * peers, so it tells them "not usable" and everybody takes the staged kernel for this one */
         t->cseq = team->xb_seq++;
-        t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, !t->captured, (t->kind == NVL_TASK_XCHG && t->use_push) ? t->push.recv_off : NULL);
+        t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, !t->captured, path_is_push(t->path) ? t->push.recv_off : NULL);
         if (t->captured) { direct = 0; t->need_xchg = 0; if (team->xb_mine->consumed < t->cseq + 1) ucc_store_release(&team->xb_mine->consumed, t->cseq + 1); }
     }
-    if (t->captured || t->kind == NVL_TASK_P2P || (ucc_list_is_empty(&team->launch_q) && (!direct || (t->published && ucc_tl_nvl_xb_ready(team, t->cseq))))) {
+    if (t->captured || (ucc_list_is_empty(&team->launch_q) && (!direct || (t->published && ucc_tl_nvl_xb_ready(team, t->cseq))))) {
         st = direct ? resolve_direct(t) : UCC_OK;
         if (st == UCC_OK) st = launch_ordered(t, s);
     } else {
@@ -540,7 +554,7 @@ static ucc_status_t nvl_triggered_post(ucc_ee_h ee, ucc_ev_t *ev, ucc_coll_task_
     ct->ee = ee;
     st = nvl_post_on(t, (cudaStream_t)ee->ee_context);
     if (st != UCC_OK) return st;
-    if (t->state == NVL_TASK_QUEUED || t->state == NVL_TASK_P2P_WAIT || (t->kind == NVL_TASK_P2P && (t->rz_pub_pending || t->rz_wait_pending))) return UCC_OK; /* the post event follows the deferred launch / publication */
+    if (t->state == NVL_TASK_QUEUED || t->state == NVL_TASK_P2P_WAIT || (t->path == NVL_PATH_P2P && (t->rz_pub_pending || t->rz_wait_pending))) return UCC_OK; /* the post event follows the deferred launch / publication */
     t->p2p_ee_done = 1;
     post_event.ev_type = UCC_EVENT_COLLECTIVE_POST; post_event.ev_context = NULL; post_event.ev_context_size = 0; post_event.req = &ct->super;
     ucc_ee_set_event_internal(ee, &post_event, &ee->event_out_queue);
@@ -586,15 +600,15 @@ static void event_put(ucc_tl_nvl_context_t *ctx, cudaEvent_t e)
     ucc_spin_unlock(&ctx->ev_lock);
     if (e) cudaEventDestroy(e);
 }
-static ucc_status_t task_alloc(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_tl_nvl_task_t **tp)
+static ucc_status_t task_alloc(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, nvl_path_t path, ucc_tl_nvl_task_t **tp)
 {
     ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
     ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
     ucc_tl_nvl_task_t *t = (ucc_tl_nvl_task_t *)ucc_mpool_get(&ctx->task_mp);
     if (!t) return UCC_ERR_NO_MEMORY;
     ucc_coll_task_init(&t->super, b, b_team);
-    t->team = team; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->want_direct = 0; t->gated = 0; t->use_push = 0; t->use_bulk = 0; t->use_ce = 0; t->use_swap = 0;
-    t->need_xchg = 0; t->direct_cached = 0; t->cached_mode = 0; t->need_src = t->need_dst = 0; t->exp_src = NULL; t->exp_dst = NULL; t->exp_src_len = t->exp_dst_len = 0; t->nblocks_direct = 0;
+    t->team = team; t->path = path; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->want_direct = 0;
+    t->need_xchg = 0; t->direct_cached = 0; t->cached_mode = 0; t->need_src = t->need_dst = 0; t->exp_src = NULL; t->exp_dst = NULL; t->exp_src_len = t->exp_dst_len = 0;
     t->nthreads = (int)ctx->cfg.nthreads;
     t->super.post = nvl_post; t->super.progress = nvl_progress; t->super.finalize = nvl_finalize; t->super.triggered_post = nvl_triggered_post;
     t->event = event_get(ctx);
@@ -621,7 +635,7 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
     ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
     ucc_coll_args_t *a = &b->args;
-    const void *src = NULL; void *dst = NULL; size_t bytes = 0;
+    const void *src = NULL; void *dst = NULL; size_t bytes = 0, copy;
     ucc_memory_type_t smt = UCC_MEMORY_TYPE_CUDA, dmt = UCC_MEMORY_TYPE_CUDA;
     ucc_tl_nvl_task_t *t;
     ucc_status_t st;
@@ -648,18 +662,17 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
         }
     }
     if (bytes && (!is_cuda(smt) || !is_cuda(dmt))) return UCC_ERR_NOT_SUPPORTED;
-    st = task_alloc(b, b_team, &t);
-    if (st != UCC_OK) return st;
-    memset(&t->u.xchg, 0, sizeof(t->u.xchg));
-    t->kind = NVL_TASK_SELF_COPY;
-    t->u.xchg.src = src; t->u.xchg.dst = dst; t->u.xchg.src_bytes = (src && dst && src != dst) ? bytes : 0;
-    t->nblocks = pick_blocks(ctx, bytes, 64 * 1024);
+    copy = (src && dst && src != dst) ? bytes : 0;
     /* from 16 MB up, cudaMemcpyAsync is the fastest copy measured (tools/selfcopy_study.py, H100 SXM 80 GB HBM3 at a 700 W
      * limit, medians of 7 rounds of 20 copies): 1 GiB 709.8 us, against 713.8 us for the best kernel candidate (non-persistent
      * TMA ring, 16 KB x 4 stages, 4 chunks per CTA), 715.5 us for the best thread copy and 732.3 us for the former persistent
      * TMA ring; 64 MB 47.7 us against 49.7 us for the thread copy below; 16 MB 8.9 us against 11.1 us.  Smaller copies, not
      * measured against it, keep the thread copy. */
-    if (t->u.xchg.src_bytes >= ((size_t)16 << 20)) t->use_ce = 1;
+    st = task_alloc(b, b_team, copy >= ((size_t)16 << 20) ? NVL_PATH_SELF_COPY_CE : NVL_PATH_SELF_COPY, &t);
+    if (st != UCC_OK) return st;
+    memset(&t->u.xchg, 0, sizeof(t->u.xchg));
+    t->u.xchg.src = src; t->u.xchg.dst = dst; t->u.xchg.src_bytes = copy;
+    t->nblocks = pick_blocks(ctx, bytes, 64 * 1024);
     *task_p = &t->super;
     return UCC_OK;
 }
@@ -667,6 +680,21 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
 /* ------------------------------------------------------------------ */
 /* reduce family                                                       */
 /* ------------------------------------------------------------------ */
+/* [p, p + len) lies in the symmetric user region (UCC_TL_NVL_USER_SIZE) after the lanes of the heap, which only an NVLS team binds
+ * to the multicast object; such memory is at the same offset on every member by contract */
+static int in_symm_region(const ucc_tl_nvl_team_t *team, const void *p, size_t len)
+{
+    const size_t user = NVL_CTX(team)->cfg.user_size;
+    const char *ub = team->heap + team->lane_stride * team->nlanes;
+    return team->nvls && user && (const char *)p >= ub && (const char *)p + len <= ub + user;
+}
+/* every reduce_scatter(v) block starts 16-byte aligned */
+static int rs_offsets_aligned(const nvl_red_args_t *r, ucc_datatype_t dt)
+{
+    for (int i = 0; i < r->team.size; i++) if ((r->rs_offset[i] * ucc_dt_size(dt)) & 15) return 0;
+    return 1;
+}
+
 typedef enum { RED_ALG_ONESHOT, RED_ALG_TWOSHOT, RED_ALG_NVLS, RED_ALG_RING, RED_ALG_RHD, RED_ALG_NVLS_PIPE } red_alg_t;
 
 static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p, red_alg_t alg)
@@ -677,10 +705,11 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
     int inplace = UCC_IS_INPLACE(*a), root = (ucc_rank_t)a->root == me;
     ucc_tl_nvl_task_t *t;
-    nvl_red_args_t *r;
+    nvl_red_args_t r;
+    nvl_path_t path;
     ucc_datatype_t dt; ucc_memory_type_t smt, dmt;
     const void *src; void *dst; size_t count, bytes;
-    int ndt, nop;
+    int ndt, nop, nb, want_direct;
     ucc_status_t st;
     if (team->self) return self_init(b, b_team, task_p);
     switch (a->coll_type) {
@@ -723,82 +752,64 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
         else need = ucc_div_round_up(count, N) * ucc_dt_size(dt);
         if (ucc_align_up(need, 16) > slice_cap) return UCC_ERR_NOT_SUPPORTED;
     }
-    st = task_alloc(b, b_team, &t);
-    if (st != UCC_OK) return st;
-    r = &t->u.red;
-    memset(r, 0, sizeof(*r));
-    r->team = team->dev; r->src = src; r->dst = dst; r->count = count; r->dt = ndt; r->op = nop; r->root = (int)a->root; r->use_nvls = (alg == RED_ALG_NVLS || alg == RED_ALG_NVLS_PIPE);
+    memset(&r, 0, sizeof(r));
+    r.team = team->dev; r.src = src; r.dst = dst; r.count = count; r.dt = ndt; r.op = nop; r.root = (int)a->root; r.use_nvls = (alg == RED_ALG_NVLS || alg == RED_ALG_NVLS_PIPE);
     switch (a->coll_type) {
-    case UCC_COLL_TYPE_ALLREDUCE: r->kind = NVL_RED_ALLREDUCE; break;
-    case UCC_COLL_TYPE_REDUCE: r->kind = NVL_RED_REDUCE; break;
+    case UCC_COLL_TYPE_ALLREDUCE: r.kind = NVL_RED_ALLREDUCE; break;
+    case UCC_COLL_TYPE_REDUCE: r.kind = NVL_RED_REDUCE; break;
     default:
-        r->kind = NVL_RED_REDUCE_SCATTER;
+        r.kind = NVL_RED_REDUCE_SCATTER;
         { size_t off = 0;
           for (ucc_rank_t i = 0; i < N; i++) {
               size_t c = a->coll_type == UCC_COLL_TYPE_REDUCE_SCATTERV ? ucc_coll_args_get_count(a, a->dst.info_v.counts, i) : ucc_buffer_block_count(count, N, i);
-              r->rs_offset[i] = off; r->rs_count[i] = c; off += c;
+              r.rs_offset[i] = off; r.rs_count[i] = c; off += c;
           }
           /* in-place: the result block stays at its offset inside the buffer */
-          if (inplace) r->dst = (char *)dst + r->rs_offset[me] * ucc_dt_size(dt); }
+          if (inplace) r.dst = (char *)dst + r.rs_offset[me] * ucc_dt_size(dt); }
         break;
     }
-    if (alg == RED_ALG_ONESHOT) { t->kind = NVL_TASK_REDUCE_ONESHOT; t->nblocks = pick_blocks(ctx, bytes, 16384); if (t->nblocks > 64) t->nblocks = 64; }
-    else if (alg == RED_ALG_RING || alg == RED_ALG_RHD) { t->kind = NVL_TASK_REDUCE_STEPS; r->sched = alg == RED_ALG_RING ? 1 : 2; t->nblocks = pick_blocks(ctx, bytes, 64 * 1024); }
-    else if (alg == RED_ALG_NVLS_PIPE) { t->kind = NVL_TASK_REDUCE_PIPE; t->nblocks = pick_blocks(ctx, bytes, 32 * 1024); }
-    else { t->kind = NVL_TASK_REDUCE_STAGED; t->nblocks = pick_blocks(ctx, bytes, 32 * 1024); }
-    /* symmetric user memory (UCC_TL_NVL_USER_SIZE): src and dst sit in the multicast-bound user region of the heap, at the same
-     * offset on every member by contract -> reduce in place through the switch, nothing staged, nothing exchanged */
-    if ((alg == RED_ALG_TWOSHOT || alg == RED_ALG_NVLS) && r->kind == NVL_RED_ALLREDUCE && team->nvls && ctx->cfg.user_size && nvl_nvls_supports(ndt, nop)) {
-        const char *ub = team->heap + team->lane_stride * team->nlanes, *ue = ub + ctx->cfg.user_size;
-        const char *s0 = (const char *)src, *d0 = (const char *)dst;
-        if (s0 >= ub && s0 + ucc_align_up(bytes, 16) <= ue && d0 >= ub && d0 + bytes <= ue && !(((uintptr_t)s0 | (uintptr_t)d0) & 15)) {
-            t->kind = NVL_TASK_REDUCE_SYMM; r->d.src[0] = s0; r->d.dst[0] = (char *)dst; r->use_nvls = 1;
-            t->nblocks = pick_blocks(ctx, bytes, 32 * 1024);
+    switch (alg) {
+    case RED_ALG_ONESHOT:
+        path = r.kind == NVL_RED_REDUCE_SCATTER ? NVL_PATH_ONESHOT_RS : NVL_PATH_ONESHOT; nb = ucc_min(pick_blocks(ctx, bytes, 16384), 64); break;
+    case RED_ALG_RING: case RED_ALG_RHD:
+        path = alg == RED_ALG_RING ? NVL_PATH_RING : NVL_PATH_RHD; r.sched = alg == RED_ALG_RING ? 1 : 2; nb = pick_blocks(ctx, bytes, 64 * 1024); break;
+    case RED_ALG_NVLS_PIPE: path = NVL_PATH_NVLS_PIPE; nb = pick_blocks(ctx, bytes, 32 * 1024); break;
+    default: path = alg == RED_ALG_NVLS ? NVL_PATH_NVLS : NVL_PATH_TWOSHOT; nb = pick_blocks(ctx, bytes, 32 * 1024); break;
+    }
+    if ((alg == RED_ALG_TWOSHOT || alg == RED_ALG_NVLS) && nvl_nvls_supports(ndt, nop)) {
+        /* symmetric user memory (UCC_TL_NVL_USER_SIZE): src and dst sit in the multicast-bound user region of the heap, at the same
+         * offset on every member by contract -> reduce in place through the switch, nothing staged, nothing exchanged */
+        if (r.kind == NVL_RED_ALLREDUCE && in_symm_region(team, src, ucc_align_up(bytes, 16)) && in_symm_region(team, dst, bytes) && !(((uintptr_t)src | (uintptr_t)dst) & 15)) {
+            path = NVL_PATH_SYMM; r.d.src[0] = src; r.d.dst[0] = dst; r.use_nvls = 1;
             /* nothing is staged here, every thread only issues multimem.ld_reduce / multimem.st, so large teams cap the grid at
              * 32 CTAs to keep the switch's request queues short (a cap chosen on an earlier GPU generation, not measured on H100) */
-            if (N > 4 && t->nblocks > 32) t->nblocks = 32;
-            *task_p = &t->super;
-            return UCC_OK;
+            if (N > 4 && nb > 32) nb = 32;
+        }
+        /* reduce_scatter(v) out of a symmetric source (the FSDP / ZeRO gradient shape): every block is reduced in the switch
+         * straight into its owner's destination, which may be any local buffer */
+        if (r.kind == NVL_RED_REDUCE_SCATTER && !inplace && !((uintptr_t)src & 15) && rs_offsets_aligned(&r, dt) && in_symm_region(team, src, ucc_align_up(bytes, 16))) {
+            path = NVL_PATH_SYMM; r.d.src[0] = src; r.d.dst[0] = NULL; r.use_nvls = 1;
+            nb = pick_blocks(ctx, bytes / N, 32 * 1024);
         }
     }
-    /* reduce_scatter(v) out of a symmetric source (the FSDP / ZeRO gradient shape): every block is reduced in the switch
-     * straight into its owner's destination, which may be any local buffer */
-    if ((alg == RED_ALG_TWOSHOT || alg == RED_ALG_NVLS) && r->kind == NVL_RED_REDUCE_SCATTER && !inplace && team->nvls && ctx->cfg.user_size && nvl_nvls_supports(ndt, nop)) {
-        const char *ub = team->heap + team->lane_stride * team->nlanes, *ue = ub + ctx->cfg.user_size;
-        const char *s0 = (const char *)src;
-        int aligned = !((uintptr_t)s0 & 15);
-        for (ucc_rank_t i = 0; i < N; i++) if ((r->rs_offset[i] * ucc_dt_size(dt)) & 15) aligned = 0;
-        if (aligned && s0 >= ub && s0 + ucc_align_up(bytes, 16) <= ue) {
-            t->kind = NVL_TASK_REDUCE_SYMM; r->d.src[0] = s0; r->d.dst[0] = NULL; r->use_nvls = 1;
-            t->nblocks = pick_blocks(ctx, bytes / N, 32 * 1024);
-            *task_p = &t->super;
-            return UCC_OK;
-        }
+    /* zero-copy, through the exchange board or from registered buffers (which also work when the board could not be set up).
+     * Every criterion below is evaluated identically on all ranks (sizes / counts are collective arguments); what only the owner
+     * knows (can the buffer be exported? is it aligned?) travels with the exchange.  The NVLS kernels stay staged: writing the
+     * result to N mapped destinations (NVL_DIRECT_DST) instead of one multicast store multiplies the bytes leaving each GPU by
+     * 1.75 on 8 members */
+    want_direct = path == NVL_PATH_TWOSHOT && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh &&
+                  (team->zcopy || (a->mask & (UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH))) &&
+                  (r.kind != NVL_RED_REDUCE_SCATTER || rs_offsets_aligned(&r, dt));
+    st = task_alloc(b, b_team, path, &t);
+    if (st != UCC_OK) return st;
+    t->u.red = r; t->nblocks = nb;
+    if (want_direct) {
+        t->want_direct = 1; t->need_src = 1; t->need_dst = r.kind != NVL_RED_REDUCE_SCATTER;
+        t->exp_src = src; t->exp_src_len = bytes;
+        t->exp_dst = r.kind == NVL_RED_REDUCE_SCATTER ? NULL : dst; t->exp_dst_len = t->exp_dst ? bytes : 0;
+        if (r.kind != NVL_RED_REDUCE) memh_direct(t, a, src, dst);
+        if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
     }
-    /* zero-copy: every criterion below is evaluated identically on all ranks (sizes / counts are collective
-     * arguments); what only the owner knows (can the buffer be exported? is it aligned?) travels with the exchange */
-    if ((alg == RED_ALG_TWOSHOT || alg == RED_ALG_NVLS) && team->zcopy && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh) {
-        /* the NVLS kernels stay staged: writing the result to N mapped destinations (NVL_DIRECT_DST) instead of one
-         * multicast store multiplies the bytes leaving each GPU by 1.75 on 8 members */
-        int mode = alg == RED_ALG_NVLS ? NVL_DIRECT_NONE : NVL_DIRECT_FULL;
-        if (mode == NVL_DIRECT_FULL && r->kind == NVL_RED_REDUCE_SCATTER)
-            for (ucc_rank_t i = 0; i < N; i++) if ((r->rs_offset[i] * ucc_dt_size(dt)) & 15) mode = NVL_DIRECT_NONE;
-        if (mode != NVL_DIRECT_NONE) {
-            t->want_direct = mode; t->nblocks_direct = t->nblocks;
-            t->need_src = mode == NVL_DIRECT_FULL; t->need_dst = r->kind != NVL_RED_REDUCE_SCATTER;
-            t->exp_src = src; t->exp_src_len = bytes;
-            t->exp_dst = r->kind == NVL_RED_REDUCE_SCATTER ? NULL : dst; t->exp_dst_len = t->exp_dst ? bytes : 0;
-        }
-    }
-    /* registered buffers make the in-place kernel available without the exchange board (also when it could not be set up) */
-    if ((alg == RED_ALG_TWOSHOT) && !t->want_direct && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh && (a->mask & (UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH))) {
-        int mode = NVL_DIRECT_FULL;
-        if (r->kind == NVL_RED_REDUCE_SCATTER) for (ucc_rank_t i = 0; i < N; i++) if ((r->rs_offset[i] * ucc_dt_size(dt)) & 15) mode = NVL_DIRECT_NONE;
-        if (mode) { t->want_direct = mode; t->nblocks_direct = t->nblocks; t->need_src = 1; t->need_dst = r->kind != NVL_RED_REDUCE_SCATTER; t->exp_src = src; t->exp_src_len = bytes;
-                    t->exp_dst = r->kind == NVL_RED_REDUCE_SCATTER ? NULL : dst; t->exp_dst_len = t->exp_dst ? bytes : 0; }
-    }
-    if (t->want_direct && r->kind != NVL_RED_REDUCE) memh_direct(t, a, src, dst);
-    if (t->want_direct && !t->direct_cached && !team->zcopy) t->want_direct = 0;
     *task_p = &t->super;
     return UCC_OK;
 }
@@ -812,18 +823,115 @@ static ucc_status_t red_init_nvls_pipe(ucc_base_coll_args_t *b, ucc_base_team_t 
 /* ------------------------------------------------------------------ */
 /* data movement family                                                */
 /* ------------------------------------------------------------------ */
-static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
+/* what every member of a data-movement collective stages and pulls; `moved`: bytes the collective moves */
+static ucc_status_t xchg_args(ucc_tl_nvl_team_t *team, const ucc_coll_args_t *a, nvl_xchg_args_t *x, size_t *moved)
+{
+    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
+    int inplace = UCC_IS_INPLACE(*a), is_root = (ucc_rank_t)a->root == me;
+    size_t dts;
+    *moved = 0;
+    switch (a->coll_type) {
+    case UCC_COLL_TYPE_ALLGATHER: {
+        size_t blk = a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype);
+        if (!is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
+        x->dst = a->dst.info.buffer; x->src = inplace ? (char *)x->dst + me * blk : a->src.info.buffer; x->src_bytes = blk;
+        for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = 0; x->pull_bytes[p] = blk; x->dst_off[p] = p * blk; }
+        *moved = blk * N; break; }
+    case UCC_COLL_TYPE_ALLGATHERV: {
+        dts = ucc_dt_size(a->dst.info_v.datatype);
+        if (!is_cuda(a->dst.info_v.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
+        x->dst = a->dst.info_v.buffer;
+        for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = 0; x->pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * dts; x->dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * dts; *moved += x->pull_bytes[p]; }
+        x->src = inplace ? (char *)x->dst + x->dst_off[me] : a->src.info.buffer; x->src_bytes = x->pull_bytes[me];
+        break; }
+    case UCC_COLL_TYPE_ALLTOALL: {
+        size_t blk = a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype);
+        if (!is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
+        x->dst = a->dst.info.buffer; x->src = inplace ? x->dst : a->src.info.buffer; x->src_bytes = blk * N; x->self_off = me * blk;
+        for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = me * blk; x->pull_bytes[p] = blk; x->dst_off[p] = p * blk; }
+        *moved = blk * N; break; }
+    case UCC_COLL_TYPE_ALLTOALLV: {
+        /* in place: the dst counts / displacements describe my buffer in both directions */
+        const ucc_coll_buffer_info_v_t *sv = inplace ? &a->dst.info_v : &a->src.info_v;
+        size_t sdt = ucc_dt_size(sv->datatype), ddt = ucc_dt_size(a->dst.info_v.datatype), end = 0;
+        if (!is_cuda(a->dst.info_v.mem_type) || !is_cuda(sv->mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        x->dst = a->dst.info_v.buffer; x->src = sv->buffer; x->publish_table = 1;
+        for (ucc_rank_t p = 0; p < N; p++) {
+            size_t so = ucc_coll_args_get_displacement(a, sv->displacements, p) * sdt, sc = ucc_coll_args_get_count(a, sv->counts, p) * sdt;
+            x->stage_off[p] = so; if (so + sc > end) end = so + sc;
+            x->pull_off[p] = NVL_XCHG_LOOKUP; x->pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * ddt;
+            x->dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * ddt; *moved += x->pull_bytes[p];
+        }
+        x->src_bytes = end; x->self_off = x->stage_off[me];
+        break; }
+    case UCC_COLL_TYPE_BCAST: {
+        size_t len = a->src.info.count * ucc_dt_size(a->src.info.datatype);
+        if (!is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        x->dst = a->src.info.buffer; x->src = a->src.info.buffer; x->src_bytes = is_root ? len : 0;
+        if (!is_root) { x->pull_off[a->root] = 0; x->pull_bytes[a->root] = len; x->dst_off[a->root] = 0; }
+        *moved = len; break; }
+    case UCC_COLL_TYPE_GATHER: {
+        size_t blk = is_root ? a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype) : a->src.info.count * ucc_dt_size(a->src.info.datatype);
+        if (is_root ? !is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type)) : !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        if (is_root) {
+            x->dst = a->dst.info.buffer; x->src = inplace ? (char *)x->dst + me * blk : a->src.info.buffer;
+            for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = 0; x->pull_bytes[p] = blk; x->dst_off[p] = p * blk; }
+        } else { x->src = a->src.info.buffer; x->src_bytes = blk; }
+        *moved = blk * N; break; }
+    case UCC_COLL_TYPE_GATHERV: {
+        if (is_root ? !is_cuda(a->dst.info_v.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type)) : !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        if (is_root) {
+            dts = ucc_dt_size(a->dst.info_v.datatype); x->dst = a->dst.info_v.buffer;
+            for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = 0; x->pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * dts; x->dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * dts; *moved += x->pull_bytes[p]; }
+            x->src = inplace ? (char *)x->dst + x->dst_off[me] : a->src.info.buffer;
+        } else { x->src = a->src.info.buffer; x->src_bytes = a->src.info.count * ucc_dt_size(a->src.info.datatype); *moved = x->src_bytes * N; }
+        break; }
+    case UCC_COLL_TYPE_SCATTER: {
+        size_t blk = is_root ? a->src.info.count / N * ucc_dt_size(a->src.info.datatype) : a->dst.info.count * ucc_dt_size(a->dst.info.datatype);
+        if (is_root ? !is_cuda(a->src.info.mem_type) || (!inplace && !is_cuda(a->dst.info.mem_type)) : !is_cuda(a->dst.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        if (is_root) { x->src = a->src.info.buffer; x->src_bytes = blk * N; x->self_off = me * blk; if (!inplace) { x->dst = a->dst.info.buffer; x->pull_bytes[me] = blk; x->dst_off[me] = 0; } }
+        else { x->dst = a->dst.info.buffer; x->pull_off[a->root] = me * blk; x->pull_bytes[a->root] = blk; x->dst_off[a->root] = 0; }
+        *moved = blk * N; break; }
+    case UCC_COLL_TYPE_SCATTERV: {
+        if (is_root ? !is_cuda(a->src.info_v.mem_type) || (!inplace && !is_cuda(a->dst.info.mem_type)) : !is_cuda(a->dst.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
+        if (is_root) {
+            size_t end = 0; dts = ucc_dt_size(a->src.info_v.datatype);
+            x->src = a->src.info_v.buffer; x->publish_table = 1;
+            for (ucc_rank_t p = 0; p < N; p++) { size_t so = ucc_coll_args_get_displacement(a, a->src.info_v.displacements, p) * dts, sc = ucc_coll_args_get_count(a, a->src.info_v.counts, p) * dts; x->stage_off[p] = so; if (so + sc > end) end = so + sc; }
+            x->src_bytes = end; x->self_off = x->stage_off[me]; *moved = end;
+            if (!inplace) { x->dst = a->dst.info.buffer; x->pull_bytes[me] = ucc_coll_args_get_count(a, a->src.info_v.counts, me) * dts; x->dst_off[me] = 0; }
+        } else { x->dst = a->dst.info.buffer; x->pull_off[a->root] = NVL_XCHG_LOOKUP; x->pull_bytes[a->root] = a->dst.info.count * ucc_dt_size(a->dst.info.datatype); x->dst_off[a->root] = 0; *moved = x->pull_bytes[a->root] * N; }
+        break; }
+    default: return UCC_ERR_NOT_SUPPORTED;
+    }
+    return UCC_OK;
+}
+
+/* Every data-movement algorithm.  `path` is the one requested; an in-place alltoall(v) takes the swap path, an allgather into a
+ * symmetric destination the multicast one, a team of one the local copy.  Whatever a path cannot serve is turned down before a
+ * task is allocated. */
+static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p, nvl_path_t path)
 {
     ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
     ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
     ucc_coll_args_t *a = &b->args;
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    int inplace = UCC_IS_INPLACE(*a), is_root = (ucc_rank_t)a->root == me;
+    ucc_coll_type_t ct = a->coll_type;
+    int inplace = UCC_IS_INPLACE(*a), a2a = ct == UCC_COLL_TYPE_ALLTOALL || ct == UCC_COLL_TYPE_ALLTOALLV;
+    int ag = ct == UCC_COLL_TYPE_ALLGATHER || ct == UCC_COLL_TYPE_ALLGATHERV;
+    /* alltoallv / gatherv / scatterv: `moved` is private to a rank, so no decision may depend on it */
+    int private_sizes = ct == UCC_COLL_TYPE_ALLTOALLV || ct == UCC_COLL_TYPE_GATHERV || ct == UCC_COLL_TYPE_SCATTERV;
     size_t cap = ctx->cfg.symmetric_size > NVL_XCHG_TABLE_BYTES ? ctx->cfg.symmetric_size - NVL_XCHG_TABLE_BYTES : 0;
+    size_t moved, off = 0, dst_len = 0;
     nvl_xchg_args_t x;
     ucc_tl_nvl_task_t *t;
-    size_t moved = 0, dts;
+    int nb;
     ucc_status_t st;
+    if (path_is_push(path) && ((!ag && !a2a) || (!team->self && (!team->zcopy || ctx->cfg.zcopy == UCC_NO)))) return UCC_ERR_NOT_SUPPORTED;
+    if (path_is_push(path) && a2a && inplace) return UCC_ERR_NOT_SUPPORTED; /* -> swap, through the score fallback */
+    if (path == NVL_PATH_PULL_NVLS && (!team->nvls || (!ag && ct != UCC_COLL_TYPE_BCAST))) return UCC_ERR_NOT_SUPPORTED;
+    if (path == NVL_PATH_PULL_RING && !ag) return UCC_ERR_NOT_SUPPORTED;
+    if (path == NVL_PATH_SWAP && !inplace) return UCC_ERR_NOT_SUPPORTED;
     if (team->self) return self_init(b, b_team, task_p);
     memset(&x, 0, sizeof(x));
     x.team = team->dev;
@@ -835,9 +943,8 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
         size_t len = a->src.info.count * ucc_dt_size(a->src.info.datatype);
         if (a->coll_type != UCC_COLL_TYPE_BCAST || a->active_set.size != 2 || !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
         if ((me != r0 && me != r1) || (root != r0 && root != r1) || r0 >= N || r1 >= N || r0 == r1) return UCC_ERR_NOT_SUPPORTED;
-        st = task_alloc(b, b_team, &t);
+        st = task_alloc(b, b_team, NVL_PATH_P2P, &t);
         if (st != UCC_OK) return st;
-        t->kind = NVL_TASK_P2P;
         memset(&t->u.p2p, 0, sizeof(t->u.p2p));
         t->u.p2p.team = team->dev; t->u.p2p.buf = a->src.info.buffer; t->u.p2p.bytes = len;
         t->u.p2p.send = me == root; t->u.p2p.peer = (int)(me == r0 ? r1 : r0);
@@ -847,251 +954,110 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
         *task_p = &t->super;
         return UCC_OK;
     }
-    switch (a->coll_type) {
-    case UCC_COLL_TYPE_ALLGATHER: {
-        size_t blk = a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype);
-        if (!is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info.buffer; x.src = inplace ? (char *)x.dst + me * blk : a->src.info.buffer; x.src_bytes = blk;
-        for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = 0; x.pull_bytes[p] = blk; x.dst_off[p] = p * blk; }
-        /* destination in the symmetric user region (same offset on every member by contract): multicast my block straight
-         * into everybody's dst - nothing staged, pulled or copied out */
-        if (team->nvls && ctx->cfg.user_size && blk && !(blk & 15) && !(((uintptr_t)x.src | (uintptr_t)x.dst) & 15)) {
-            const char *ub = team->heap + team->lane_stride * team->nlanes, *ue = ub + ctx->cfg.user_size, *d0 = (const char *)x.dst;
-            if (d0 >= ub && d0 + blk * N <= ue) {
-                st = task_alloc(b, b_team, &t);
-                if (st != UCC_OK) return st;
-                x.push_off = (size_t)me * blk;
-                t->kind = NVL_TASK_AG_SYMM; t->u.xchg = x;
-                t->nblocks = pick_blocks(ctx, blk, 32 * 1024);
-                *task_p = &t->super;
-                return UCC_OK;
+    st = xchg_args(team, a, &x, &moved);
+    if (st != UCC_OK) return st;
+    if (ct == UCC_COLL_TYPE_ALLGATHER && x.src_bytes && !(x.src_bytes & 15) && !(((uintptr_t)x.src | (uintptr_t)x.dst) & 15) && in_symm_region(team, x.dst, x.src_bytes * N)) {
+        /* destination in the symmetric user region: multicast my block straight into everybody's dst - nothing staged, pulled
+         * or copied out */
+        path = NVL_PATH_AG_SYMM; x.push_off = (size_t)me * x.src_bytes;
+        nb = pick_blocks(ctx, x.src_bytes, 32 * 1024);
+    } else {
+        /* the staged payload must fit the heap (every rank evaluates the same bound for symmetric colls;
+         * v-variants that exceed it are rejected on the ranks that notice -> use a size hint via TUNE to avoid) */
+        if (x.src_bytes > cap) return UCC_ERR_NOT_SUPPORTED;
+        /* the grid must be the same on every rank (blocks pair up through per-block flags): a fixed one where `moved` is private */
+        nb = private_sizes ? (int)ucc_min(ctx->cfg.max_blocks, (ctx->cfg.nblocks != UCC_UUNITS_AUTO && ctx->cfg.nblocks > 0) ? ctx->cfg.nblocks : 128u)
+                           : pick_blocks(ctx, moved, 64 * 1024);
+        /* the zero-copy pull must never run in place: the peers overwrite the buffer it reads */
+        if (inplace && a2a) path = NVL_PATH_SWAP;
+        if (path == NVL_PATH_PULL_NVLS) {
+            /* every rank multicasts its block once (multimem.st) to its offset in every heap; every allgatherv member knows all
+             * counts, so the layout agrees everywhere */
+            if (ct == UCC_COLL_TYPE_BCAST) { x.push_off = 0; off = x.src_bytes; }
+            else for (ucc_rank_t p = 0; p < N; p++) { if (p == me) x.push_off = off; x.pull_off[p] = off; off += ucc_align_up(x.pull_bytes[p] ? x.pull_bytes[p] : (p == me ? x.src_bytes : 0), 16); }
+            if (off > cap) return UCC_ERR_NOT_SUPPORTED;
+            x.use_mc = 1;
+        }
+        if (path == NVL_PATH_PULL_RING) { /* same heap layout as the nvls variant */
+            for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = off; off += ucc_align_up(x.pull_bytes[p], 16); }
+            if (off > cap) return UCC_ERR_NOT_SUPPORTED;
+            x.ring = 1;
+            for (ucc_rank_t p = 0; p < N; p++) { x.ring_order[p] = (int)team->ring_order[p]; if (team->ring_order[p] == me) x.ring_pos = (int)p; }
+        }
+        /* push alltoallv: one landing-offset table per block at the start of the data region */
+        if (path_is_push(path) && ct == UCC_COLL_TYPE_ALLTOALLV && (size_t)nb * NVL_MAX_PEERS * sizeof(uint64_t) > ctx->cfg.symmetric_size) return UCC_ERR_NOT_SUPPORTED;
+        if (path == NVL_PATH_PUSH) {
+            /* data mover: the TMA engine for big transfers (the choice may only depend on what every member knows - sizes of
+             * alltoallv are private, it always takes it) */
+            size_t total = 0;
+            for (ucc_rank_t p = 0; p < N; p++) total += x.pull_bytes[p];
+            if (ctx->cfg.bulk != UCC_NO && (ct == UCC_COLL_TYPE_ALLTOALLV || total >= ctx->cfg.bulk_thresh)) {
+                path = NVL_PATH_PUSH_BULK; nb = (int)ucc_max(1u, ucc_min(ctx->cfg.bulk_ctas, ctx->cfg.max_blocks));
             }
         }
-        moved = blk * N; break; }
-    case UCC_COLL_TYPE_ALLGATHERV: {
-        dts = ucc_dt_size(a->dst.info_v.datatype);
-        if (!is_cuda(a->dst.info_v.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info_v.buffer;
-        for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = 0; x.pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * dts; x.dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * dts; moved += x.pull_bytes[p]; }
-        x.src = inplace ? (char *)x.dst + x.dst_off[me] : a->src.info.buffer; x.src_bytes = x.pull_bytes[me];
-        break; }
-    case UCC_COLL_TYPE_ALLTOALL: {
-        size_t blk = a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype);
-        if (!is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type))) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info.buffer; x.src = inplace ? x.dst : a->src.info.buffer; x.src_bytes = blk * N; x.self_off = me * blk;
-        for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = me * blk; x.pull_bytes[p] = blk; x.dst_off[p] = p * blk; }
-        moved = blk * N; break; }
-    case UCC_COLL_TYPE_ALLTOALLV: {
-        /* in place: the dst counts / displacements describe my buffer in both directions */
-        const ucc_coll_buffer_info_v_t *sv = inplace ? &a->dst.info_v : &a->src.info_v;
-        size_t sdt = ucc_dt_size(sv->datatype), ddt = ucc_dt_size(a->dst.info_v.datatype), end = 0;
-        if (!is_cuda(a->dst.info_v.mem_type) || !is_cuda(sv->mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->dst.info_v.buffer; x.src = sv->buffer; x.publish_table = 1;
-        for (ucc_rank_t p = 0; p < N; p++) {
-            size_t so = ucc_coll_args_get_displacement(a, sv->displacements, p) * sdt, sc = ucc_coll_args_get_count(a, sv->counts, p) * sdt;
-            x.stage_off[p] = so; if (so + sc > end) end = so + sc;
-            x.pull_off[p] = NVL_XCHG_LOOKUP; x.pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * ddt;
-            x.dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * ddt; moved += x.pull_bytes[p];
-        }
-        x.src_bytes = end; x.self_off = x.stage_off[me];
-        break; }
-    case UCC_COLL_TYPE_BCAST: {
-        size_t len = a->src.info.count * ucc_dt_size(a->src.info.datatype);
-        if (!is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        x.dst = a->src.info.buffer; x.src = a->src.info.buffer; x.src_bytes = is_root ? len : 0;
-        if (!is_root) { x.pull_off[a->root] = 0; x.pull_bytes[a->root] = len; x.dst_off[a->root] = 0; }
-        moved = len; break; }
-    case UCC_COLL_TYPE_GATHER: {
-        size_t blk = is_root ? a->dst.info.count / N * ucc_dt_size(a->dst.info.datatype) : a->src.info.count * ucc_dt_size(a->src.info.datatype);
-        if (is_root ? !is_cuda(a->dst.info.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type)) : !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        if (is_root) {
-            x.dst = a->dst.info.buffer; x.src = inplace ? (char *)x.dst + me * blk : a->src.info.buffer;
-            for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = 0; x.pull_bytes[p] = blk; x.dst_off[p] = p * blk; }
-        } else { x.src = a->src.info.buffer; x.src_bytes = blk; }
-        moved = blk * N; break; }
-    case UCC_COLL_TYPE_GATHERV: {
-        if (is_root ? !is_cuda(a->dst.info_v.mem_type) || (!inplace && !is_cuda(a->src.info.mem_type)) : !is_cuda(a->src.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        if (is_root) {
-            dts = ucc_dt_size(a->dst.info_v.datatype); x.dst = a->dst.info_v.buffer;
-            for (ucc_rank_t p = 0; p < N; p++) { x.pull_off[p] = 0; x.pull_bytes[p] = ucc_coll_args_get_count(a, a->dst.info_v.counts, p) * dts; x.dst_off[p] = ucc_coll_args_get_displacement(a, a->dst.info_v.displacements, p) * dts; moved += x.pull_bytes[p]; }
-            x.src = inplace ? (char *)x.dst + x.dst_off[me] : a->src.info.buffer;
-        } else { x.src = a->src.info.buffer; x.src_bytes = a->src.info.count * ucc_dt_size(a->src.info.datatype); moved = x.src_bytes * N; }
-        break; }
-    case UCC_COLL_TYPE_SCATTER: {
-        size_t blk = is_root ? a->src.info.count / N * ucc_dt_size(a->src.info.datatype) : a->dst.info.count * ucc_dt_size(a->dst.info.datatype);
-        if (is_root ? !is_cuda(a->src.info.mem_type) || (!inplace && !is_cuda(a->dst.info.mem_type)) : !is_cuda(a->dst.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        if (is_root) { x.src = a->src.info.buffer; x.src_bytes = blk * N; x.self_off = me * blk; if (!inplace) { x.dst = a->dst.info.buffer; x.pull_bytes[me] = blk; x.dst_off[me] = 0; } }
-        else { x.dst = a->dst.info.buffer; x.pull_off[a->root] = me * blk; x.pull_bytes[a->root] = blk; x.dst_off[a->root] = 0; }
-        moved = blk * N; break; }
-    case UCC_COLL_TYPE_SCATTERV: {
-        if (is_root ? !is_cuda(a->src.info_v.mem_type) || (!inplace && !is_cuda(a->dst.info.mem_type)) : !is_cuda(a->dst.info.mem_type)) return UCC_ERR_NOT_SUPPORTED;
-        if (is_root) {
-            size_t end = 0; dts = ucc_dt_size(a->src.info_v.datatype);
-            x.src = a->src.info_v.buffer; x.publish_table = 1;
-            for (ucc_rank_t p = 0; p < N; p++) { size_t so = ucc_coll_args_get_displacement(a, a->src.info_v.displacements, p) * dts, sc = ucc_coll_args_get_count(a, a->src.info_v.counts, p) * dts; x.stage_off[p] = so; if (so + sc > end) end = so + sc; }
-            x.src_bytes = end; x.self_off = x.stage_off[me]; moved = end;
-            if (!inplace) { x.dst = a->dst.info.buffer; x.pull_bytes[me] = ucc_coll_args_get_count(a, a->src.info_v.counts, me) * dts; x.dst_off[me] = 0; }
-        } else { x.dst = a->dst.info.buffer; x.pull_off[a->root] = NVL_XCHG_LOOKUP; x.pull_bytes[a->root] = a->dst.info.count * ucc_dt_size(a->dst.info.datatype); x.dst_off[a->root] = 0; moved = x.pull_bytes[a->root] * N; }
-        break; }
-    default: return UCC_ERR_NOT_SUPPORTED;
+        if (path == NVL_PATH_PUSH_CE) nb = 1;
     }
-    /* the staged payload must fit the heap (every rank evaluates the same bound for symmetric colls;
-     * v-variants that exceed it are rejected on the ranks that notice -> use a size hint via TUNE to avoid) */
-    if (x.src_bytes > cap) return UCC_ERR_NOT_SUPPORTED;
-    st = task_alloc(b, b_team, &t);
+    st = task_alloc(b, b_team, path, &t);
     if (st != UCC_OK) return st;
-    t->kind = NVL_TASK_XCHG; t->u.xchg = x;
-    t->nblocks = pick_blocks(ctx, moved, 64 * 1024);
-    /* the grid must be the same on every rank (blocks pair up through per-block flags), but for alltoallv / gatherv /
-     * scatterv `moved` is private to a rank: use a fixed grid for those */
-    if (a->coll_type == UCC_COLL_TYPE_ALLTOALLV || a->coll_type == UCC_COLL_TYPE_GATHERV || a->coll_type == UCC_COLL_TYPE_SCATTERV)
-        t->nblocks = (int)ucc_min(ctx->cfg.max_blocks, (ctx->cfg.nblocks != UCC_UUNITS_AUTO && ctx->cfg.nblocks > 0) ? ctx->cfg.nblocks : 128u);
-    if (inplace && (a->coll_type == UCC_COLL_TYPE_ALLTOALL || a->coll_type == UCC_COLL_TYPE_ALLTOALLV)) {
+    t->u.xchg = x; t->nblocks = nb;
+    if (path == NVL_PATH_SWAP && ctx->cfg.zcopy != UCC_NO && (size_t)nb * NVL_SWAP_TABLE_BYTES <= ctx->cfg.symmetric_size) {
         /* the buffers travel over the exchange board (or come from registrations) as destinations: the swap kernel reads and
-         * writes them in place, and when they do not resolve, launch_swap stages.  The zero-copy pull (need_src) must never run
-         * in place: the peers overwrite the buffer it reads. */
-        t->use_swap = 1;
-        if (ctx->cfg.zcopy != UCC_NO && (size_t)t->nblocks * NVL_SWAP_TABLE_BYTES <= ctx->cfg.symmetric_size) {
-            t->want_direct = NVL_DIRECT_FULL; t->need_src = 0; t->need_dst = 1;
-            t->exp_dst = x.dst; t->exp_dst_len = x.src_bytes;
-            memh_direct(t, a, NULL, x.dst);
-            if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
+         * writes them in place, and when they do not resolve, launch_swap stages */
+        t->want_direct = 1; t->need_dst = 1;
+        t->exp_dst = x.dst; t->exp_dst_len = x.src_bytes;
+        memh_direct(t, a, NULL, x.dst);
+        if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
+    }
+    /* (private sizes: always - the choice may only depend on what every rank knows, and staging a skewed alltoallv through the
+     * heap was 2.4x slower than NCCL at 16 MB on 4 GPUs; below ~4 MB the host-side exchange costs more than the staging copy) */
+    if (path == NVL_PATH_PULL && team->zcopy && ctx->cfg.zcopy != UCC_NO &&
+        (private_sizes || moved >= (ctx->cfg.zcopy == UCC_YES ? ctx->cfg.zcopy_thresh : ucc_max(ctx->cfg.zcopy_thresh, (size_t)4 << 20)))) {
+        t->want_direct = 1; t->need_src = 1;
+        t->exp_src = x.src_bytes ? x.src : NULL; t->exp_src_len = x.src_bytes;
+    }
+    if (path_is_push(path)) {
+        /* the destinations travel over the exchange board and every rank stores its blocks straight into them; if a destination
+         * cannot be mapped the task runs the staged pull */
+        t->push.lookup = 0;
+        for (ucc_rank_t p = 0; p < N; p++) {
+            t->push.recv_off[p] = x.dst_off[p];
+            if (ct == UCC_COLL_TYPE_ALLTOALLV) {
+                /* what I send is described by MY send counts / displacements (x.stage_off); where it lands only the receiver knows:
+                 * it publishes recv_off[] on the device and the senders look their entry up (the mirror image of the pull kernel's table) */
+                size_t sdt = ucc_dt_size(a->src.info_v.datatype);
+                t->push.send_off[p] = x.stage_off[p]; t->push.send_bytes[p] = ucc_coll_args_get_count(a, a->src.info_v.counts, p) * sdt;
+                t->push.land_off[p] = x.dst_off[me]; t->push.lookup = 1;
+            } else if (ct == UCC_COLL_TYPE_ALLTOALL) { t->push.send_off[p] = x.dst_off[p]; t->push.send_bytes[p] = x.pull_bytes[p]; t->push.land_off[p] = x.dst_off[me]; }
+            else { t->push.send_off[p] = 0; t->push.send_bytes[p] = x.pull_bytes[me]; t->push.land_off[p] = x.dst_off[me]; } /* my block, at my displacement, in everybody's dst */
+            if (x.dst_off[p] + x.pull_bytes[p] > dst_len) dst_len = x.dst_off[p] + x.pull_bytes[p];
         }
-    } else if (team->zcopy && ctx->cfg.zcopy != UCC_NO) {
-        /* `moved` is the same number on every rank except for the v-collectives whose counts are private to a
-         * rank (alltoallv, gatherv, scatterv): those only go zero-copy when it is forced, size-independently */
-        int symmetric = a->coll_type != UCC_COLL_TYPE_ALLTOALLV && a->coll_type != UCC_COLL_TYPE_GATHERV && a->coll_type != UCC_COLL_TYPE_SCATTERV;
-        /* (asymmetric ones: always - the choice may only depend on what every rank knows, and staging a skewed
-         * alltoallv through the heap was 2.4x slower than NCCL at 16 MB on 4 GPUs) */
-        if (symmetric ? moved >= (ctx->cfg.zcopy == UCC_YES ? ctx->cfg.zcopy_thresh : ucc_max(ctx->cfg.zcopy_thresh, (size_t)4 << 20)) : 1) { /* below ~4 MB the host-side exchange costs more than the staging copy */
-            t->want_direct = NVL_DIRECT_FULL; t->need_src = 1; t->need_dst = 0;
-            t->exp_src = x.src_bytes ? x.src : NULL; t->exp_src_len = x.src_bytes;
-        }
+        t->want_direct = 1; t->need_dst = 1;
+        t->exp_dst = x.dst; t->exp_dst_len = dst_len;
     }
     *task_p = &t->super;
     return UCC_OK;
 }
-
-/* zero-copy PUSH allgather(v) / alltoall (kernels/nvl_push.cu): the destinations travel over the exchange board and every rank
- * stores its blocks straight into them; if a destination cannot be mapped the task falls back to the staged pull it also is */
-static ucc_status_t xchg_init_push(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
-{
-    ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
-    ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
-    ucc_coll_args_t *a = &b->args;
-    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    ucc_coll_type_t ct = a->coll_type;
-    ucc_tl_nvl_task_t *t;
-    nvl_xchg_args_t *x;
-    size_t dst_len = 0;
-    ucc_status_t st;
-    if (ct != UCC_COLL_TYPE_ALLGATHER && ct != UCC_COLL_TYPE_ALLGATHERV && ct != UCC_COLL_TYPE_ALLTOALL && ct != UCC_COLL_TYPE_ALLTOALLV) return UCC_ERR_NOT_SUPPORTED;
-    if (!team->self && (!team->zcopy || ctx->cfg.zcopy == UCC_NO)) return UCC_ERR_NOT_SUPPORTED;
-    if ((ct == UCC_COLL_TYPE_ALLTOALL || ct == UCC_COLL_TYPE_ALLTOALLV) && UCC_IS_INPLACE(*a)) return UCC_ERR_NOT_SUPPORTED; /* -> swap, through the score fallback */
-    st = xchg_init(b, b_team, task_p);
-    if (st != UCC_OK) return st;
-    t = ucc_derived_of(*task_p, ucc_tl_nvl_task_t); x = &t->u.xchg;
-    if (t->kind != NVL_TASK_XCHG) return UCC_OK; /* symmetric destination / single member: nothing to add */
-    t->push.lookup = 0;
-    for (ucc_rank_t p = 0; p < N; p++) {
-        t->push.recv_off[p] = x->dst_off[p];
-        if (ct == UCC_COLL_TYPE_ALLTOALLV) {
-            /* what I send is described by MY send counts / displacements (x->stage_off); where it lands only the receiver knows:
-             * it publishes recv_off[] on the device and the senders look their entry up (the mirror image of the pull kernel's table) */
-            size_t sdt = ucc_dt_size(a->src.info_v.datatype);
-            t->push.send_off[p] = x->stage_off[p]; t->push.send_bytes[p] = ucc_coll_args_get_count(a, a->src.info_v.counts, p) * sdt;
-            t->push.land_off[p] = x->dst_off[me]; t->push.lookup = 1;
-        } else if (ct == UCC_COLL_TYPE_ALLTOALL) { t->push.send_off[p] = x->dst_off[p]; t->push.send_bytes[p] = x->pull_bytes[p]; t->push.land_off[p] = x->dst_off[me]; }
-        else { t->push.send_off[p] = 0; t->push.send_bytes[p] = x->pull_bytes[me]; t->push.land_off[p] = x->dst_off[me]; } /* my block, at my displacement, in everybody's dst */
-        if (x->dst_off[p] + x->pull_bytes[p] > dst_len) dst_len = x->dst_off[p] + x->pull_bytes[p];
-    }
-    /* alltoallv: one landing-offset table per block at the start of the data region */
-    if (t->push.lookup && (size_t)t->nblocks * NVL_MAX_PEERS * sizeof(uint64_t) > ctx->cfg.symmetric_size) { (*task_p)->finalize(*task_p); *task_p = NULL; return UCC_ERR_NOT_SUPPORTED; }
-    t->use_push = 1;
-    /* data mover: the TMA engine for big transfers (the choice may only depend on what every member knows - sizes of the
-     * v-collectives are private, those always take it) */
-    { size_t total = 0; int symmetric = ct == UCC_COLL_TYPE_ALLGATHER || ct == UCC_COLL_TYPE_ALLTOALL || ct == UCC_COLL_TYPE_ALLGATHERV;
-      for (ucc_rank_t p = 0; p < N; p++) total += x->pull_bytes[p];
-      t->use_bulk = ctx->cfg.bulk != UCC_NO && (symmetric ? total >= ctx->cfg.bulk_thresh : 1);
-      if (t->use_bulk) t->nblocks = (int)ucc_max(1u, ucc_min(ctx->cfg.bulk_ctas, ctx->cfg.max_blocks)); }
-    t->want_direct = NVL_DIRECT_FULL; t->need_src = 0; t->need_dst = 1;
-    t->exp_src = NULL; t->exp_src_len = 0; t->exp_dst = x->dst; t->exp_dst_len = dst_len;
-    return UCC_OK;
-}
-
-/* copy-engine push exchange: same buffer resolution as `push`, the copies are DMAs issued by the host (see nvl_launch) */
-static ucc_status_t xchg_init_ce(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
-{
-    ucc_tl_nvl_task_t *t;
-    ucc_status_t st = xchg_init_push(b, b_team, task_p);
-    if (st != UCC_OK) return st;
-    t = ucc_derived_of(*task_p, ucc_tl_nvl_task_t);
-    if (t->kind != NVL_TASK_XCHG) return UCC_OK;
-    t->use_ce = 1; t->use_bulk = 0; t->nblocks = 1;
-    return UCC_OK;
-}
-
+static ucc_status_t xchg_init_pull(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_PULL); }
+/* zero-copy push allgather(v) / alltoall(v) (kernels/nvl_push.cu), moved by threads or, from BULK_THRESH, by TMA bulk copies */
+static ucc_status_t xchg_init_push(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_PUSH); }
+/* the same buffer resolution as `push`, the copies are DMAs issued by the host (see launch_push) */
+static ucc_status_t xchg_init_ce(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_PUSH_CE); }
 /* in-place alltoall(v) only (kernels/nvl_swap.cu): what `pull` also does with such a request, under a name TUNE can select */
-static ucc_status_t xchg_init_swap(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
-{
-    if (!UCC_IS_INPLACE(b->args)) return UCC_ERR_NOT_SUPPORTED;
-    return xchg_init(b, b_team, task_p);
-}
-
-/* allgather(v) / bcast through the switch: every rank multicasts its block once (multimem.st), everybody then
- * copies out of its OWN heap.  Same bytes into every GPU as the pull variant, 1/(N-1) of the bytes out. */
-static ucc_status_t xchg_init_nvls(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
-{
-    ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
-    ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
-    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    ucc_coll_type_t ct = b->args.coll_type;
-    size_t cap = ctx->cfg.symmetric_size > NVL_XCHG_TABLE_BYTES ? ctx->cfg.symmetric_size - NVL_XCHG_TABLE_BYTES : 0, off = 0;
-    ucc_tl_nvl_task_t *t;
-    nvl_xchg_args_t *x;
-    ucc_status_t st;
-    if (!team->nvls || (ct != UCC_COLL_TYPE_ALLGATHER && ct != UCC_COLL_TYPE_ALLGATHERV && ct != UCC_COLL_TYPE_BCAST)) return UCC_ERR_NOT_SUPPORTED;
-    st = xchg_init(b, b_team, task_p);
-    if (st != UCC_OK) return st;
-    t = ucc_derived_of(*task_p, ucc_tl_nvl_task_t); x = &t->u.xchg;
-    if (t->kind != NVL_TASK_XCHG) return UCC_OK; /* symmetric-destination allgather or single-member copy: already complete */
-    t->want_direct = 0;
-    if (ct == UCC_COLL_TYPE_BCAST) { x->push_off = 0; off = x->src_bytes; }
-    else for (ucc_rank_t p = 0; p < N; p++) { if (p == me) x->push_off = off; x->pull_off[p] = off; off += ucc_align_up(x->pull_bytes[p] ? x->pull_bytes[p] : (p == me ? x->src_bytes : 0), 16); }
-    /* NOTE for allgatherv every rank knows all counts, so `off` (and the decisions below) agree everywhere */
-    if (off > cap) { (*task_p)->finalize(*task_p); *task_p = NULL; return UCC_ERR_NOT_SUPPORTED; }
-    x->use_mc = 1;
-    return UCC_OK;
-}
-/* ring allgather(v): same heap layout as the nvls variant, N-1 neighbour-to-neighbour steps inside one kernel */
-static ucc_status_t xchg_init_ring(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
-{
-    ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
-    ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
-    ucc_rank_t N = UCC_TL_TEAM_SIZE(team);
-    size_t cap = ctx->cfg.symmetric_size > NVL_XCHG_TABLE_BYTES ? ctx->cfg.symmetric_size - NVL_XCHG_TABLE_BYTES : 0, off = 0;
-    ucc_tl_nvl_task_t *t; nvl_xchg_args_t *x; ucc_status_t st;
-    if (b->args.coll_type != UCC_COLL_TYPE_ALLGATHER && b->args.coll_type != UCC_COLL_TYPE_ALLGATHERV) return UCC_ERR_NOT_SUPPORTED;
-    st = xchg_init(b, b_team, task_p);
-    if (st != UCC_OK) return st;
-    t = ucc_derived_of(*task_p, ucc_tl_nvl_task_t); x = &t->u.xchg;
-    if (t->kind != NVL_TASK_XCHG) return UCC_OK; /* symmetric-destination allgather or single-member copy: already complete */
-    t->want_direct = 0;
-    for (ucc_rank_t p = 0; p < N; p++) { x->pull_off[p] = off; off += ucc_align_up(x->pull_bytes[p], 16); }
-    if (off > cap) { (*task_p)->finalize(*task_p); *task_p = NULL; return UCC_ERR_NOT_SUPPORTED; }
-    x->ring = 1;
-    for (ucc_rank_t p = 0; p < N; p++) { x->ring_order[p] = (int)team->ring_order[p]; if (team->ring_order[p] == UCC_TL_TEAM_RANK(team)) x->ring_pos = (int)p; }
-    return UCC_OK;
-}
+static ucc_status_t xchg_init_swap(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_SWAP); }
+/* allgather(v) / bcast through the switch: every rank multicasts its block once (multimem.st), everybody then copies out of its
+ * OWN heap.  Same bytes into every GPU as the pull variant, 1/(N-1) of the bytes out. */
+static ucc_status_t xchg_init_nvls(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_PULL_NVLS); }
+/* ring allgather(v): N-1 neighbour-to-neighbour steps inside one kernel */
+static ucc_status_t xchg_init_ring(ucc_base_coll_args_t *b, ucc_base_team_t *t, ucc_coll_task_t **p) { return xchg_init(b, t, p, NVL_PATH_PULL_RING); }
 
 static ucc_status_t barrier_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, ucc_coll_task_t **task_p)
 {
     ucc_tl_nvl_task_t *t;
     ucc_status_t st;
     if (ucc_derived_of(b_team, ucc_tl_nvl_team_t)->self) return self_init(b, b_team, task_p);
-    st = task_alloc(b, b_team, &t);
+    st = task_alloc(b, b_team, NVL_PATH_BARRIER, &t);
     if (st != UCC_OK) return st;
-    t->kind = NVL_TASK_BARRIER; t->nblocks = 1;
+    t->nblocks = 1;
     memset(&t->u.red, 0, sizeof(t->u.red)); t->u.red.team = ucc_derived_of(b_team, ucc_tl_nvl_team_t)->dev;
     *task_p = &t->super;
     return UCC_OK;
@@ -1117,15 +1083,15 @@ static const nvl_alg_t algs_rs[] = {
 static const nvl_alg_t algs_red[] = {
     {"twoshot", "stage + pull-reduce own slice over NVLink", red_init_twoshot},
     {"nvls", "stage + multimem.ld_reduce own slice in the NVSwitch", red_init_nvls}, {NULL}};
-static const nvl_alg_t algs_xchg[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init}, {NULL}};
-static const nvl_alg_t algs_xchg_mc[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init},
+static const nvl_alg_t algs_xchg[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init_pull}, {NULL}};
+static const nvl_alg_t algs_xchg_mc[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init_pull},
     {"nvls", "multicast the own block into every member's heap with multimem.st, copy out locally", xchg_init_nvls}, {NULL}};
-static const nvl_alg_t algs_ag[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init},
+static const nvl_alg_t algs_ag[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init_pull},
     {"nvls", "multicast the own block into every member's heap with multimem.st, copy out locally", xchg_init_nvls},
     {"ring", "N-1 neighbour-to-neighbour pull steps through the heaps, one kernel", xchg_init_ring},
     {"push", "zero-copy push: every rank stores its block straight into the members' mapped destinations (TMA bulk copies from BULK_THRESH)", xchg_init_push},
     {"ce", "zero-copy push by the copy engines: cudaMemcpyAsync into the members' mapped destinations between two barrier kernels", xchg_init_ce}, {NULL}};
-static const nvl_alg_t algs_a2a[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init},
+static const nvl_alg_t algs_a2a[] = {{"pull", "stage once, every peer pulls its part over NVLink", xchg_init_pull},
     {"push", "zero-copy push: every rank stores block p straight into member p's mapped destination; alltoallv looks the landing offset up in a table the receiver publishes on the device", xchg_init_push},
     {"ce", "zero-copy push by the copy engines (reference ALLTOALL_USE_COPY_ENGINE): one cudaMemcpyAsync per peer between two barrier kernels", xchg_init_ce},
     {"swap", "in place only: every pair of members swaps its two regions straight between their mapped buffers, no staging (staged pull when a buffer cannot be mapped)", xchg_init_swap}, {NULL}};

@@ -155,7 +155,6 @@ static void team_release(ucc_tl_nvl_team_t *team)
     }
     if (team->mc_fd >= 0) { close(team->mc_fd); team->mc_fd = -1; }
     if (team->host_err) { cudaFreeHost(team->host_err); team->host_err = NULL; }
-    if (team->gates) { cudaFree(team->gates); team->gates = NULL; }
     for (unsigned l = 0; l < NVL_MAX_LANES; l++) if (team->order_event[l]) { cudaEventDestroy(team->order_event[l]); team->order_event[l] = NULL; }
     ucc_tl_nvl_xb_release(team);
     if (team->oob_internal) { ucc_internal_oob_finalize(&team->oob); team->oob_internal = 0; }
@@ -313,11 +312,9 @@ static ucc_status_t team_finish(ucc_tl_nvl_team_t *team)
     CUDA_CHECK(cudaStreamCreateWithFlags(&team->stream, cudaStreamNonBlocking));
     CUDA_CHECK(cudaHostAlloc((void **)&team->host_err, sizeof(uint32_t), cudaHostAllocMapped));
     *team->host_err = 0;
-    CUDA_CHECK(cudaMalloc((void **)&team->gates, NVL_GATE_SLOTS * sizeof(uint32_t)));
-    CUDA_CHECK(cudaMemset(team->gates, 0, NVL_GATE_SLOTS * sizeof(uint32_t)));
     for (unsigned l = 0; l < team->nlanes; l++) CUDA_CHECK(cudaEventCreateWithFlags(&team->order_event[l], cudaEventDisableTiming));
     ucc_list_head_init(&team->launch_q); ucc_spinlock_init(&team->launch_lock);
-    memset(team->last_stream, 0, sizeof(team->last_stream)); memset(team->last_event, 0, sizeof(team->last_event)); team->lane_seq = 0; team->gate_seq = 0; team->xb_seq = 0;
+    memset(team->last_stream, 0, sizeof(team->last_stream)); memset(team->last_event, 0, sizeof(team->last_event)); team->lane_seq = 0; team->xb_seq = 0;
     memset(&team->dev, 0, sizeof(team->dev));
     team->dev.rank = (int)UCC_TL_TEAM_RANK(team); team->dev.size = (int)N;
     for (ucc_rank_t p = 0; p < N; p++) team->dev.heap[p] = team->peer_va[p];
