@@ -198,12 +198,19 @@ template <typename A> struct IsIntAcc { static constexpr bool v = true; };
 template <> struct IsIntAcc<float> { static constexpr bool v = false; };
 template <> struct IsIntAcc<double> { static constexpr bool v = false; };
 template <typename R> struct IsIntAcc<nvl_complex<R>> { static constexpr bool v = false; };
+/* 1/N in the precision R scales in: the caller's float 1/N for float, 1/N computed in double for double (the float 1/N is off by up
+ * to 2^-25 relative, some 2^28 ulp of a double) */
+template <typename R> NVL_DEV R inv_n_as(float inv_n, int n)
+{
+    if constexpr (sizeof(R) == sizeof(double)) return 1.0 / (double)n;
+    else return (R)inv_n;
+}
 template <int OP, typename A> NVL_DEV A avg_scale(A x, float inv_n, int n)
 {
     if (OP != NVL_OP_AVG) return x;
     if constexpr (IsIntAcc<A>::v) return n > 1 ? (A)(x / (A)n) : x;
-    else if constexpr (IsComplex<A>::v) return {x.re * inv_n, x.im * inv_n}; /* both components by the factor f32 / f64 use */
-    else return (A)(x * (A)inv_n);
+    else if constexpr (IsComplex<A>::v) { const auto s = inv_n_as<decltype(x.re)>(inv_n, n); return {x.re * s, x.im * s}; } /* as the real type */
+    else return x * inv_n_as<A>(inv_n, n);
 }
 
 /* accumulator for one 16-byte vector of T */

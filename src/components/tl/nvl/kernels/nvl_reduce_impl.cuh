@@ -77,10 +77,12 @@ static __device__ __forceinline__ void oneshot_body(const nvl_red_args_t &a, nvl
     __syncthreads();
     const char *mybase = t.heap[me] + NVL_LL_OFFSET + slot;
     for (size_t v = v0 + threadIdx.x; v < v1; v += blockDim.x) {
+        /* reduced in rank order 0..N-1 on every rank (my own vector at position me), so all ranks get the same bits: a rotated
+         * order per rank rounds floating-point sums differently on every rank and lets MAX / MIN of NaN or +-0 differ by rank */
+        const uint4 own = load_src_vec<T>(src, v * E, n, sal);
         uint4 x[NVL_MAX_PEERS];
-        x[0] = load_src_vec<T>(src, v * E, n, sal);
 #pragma unroll
-        for (int i = 1; i < NVL_MAX_PEERS; i++) if (i < N) { int p = me + i; if (p >= N) p -= N; x[i] = ld_peer_v4(mybase + (size_t)p * NVL_LL_MAX + v * 16); }
+        for (int i = 0; i < NVL_MAX_PEERS; i++) if (i < N) x[i] = i == me ? own : ld_peer_v4(mybase + (size_t)i * NVL_LL_MAX + v * 16);
         VecAcc<T, OP> acc; acc.set(x[0]);
 #pragma unroll
         for (int i = 1; i < NVL_MAX_PEERS; i++) if (i < N) acc.add(x[i]);
