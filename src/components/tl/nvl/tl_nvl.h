@@ -198,6 +198,20 @@ typedef enum {
     NVL_PATH_NUM
 } nvl_path_t;
 typedef enum { NVL_TASK_LAUNCHED, NVL_TASK_QUEUED, NVL_TASK_P2P_WAIT /* send waiting for its turn / for the receiver's buffer */ } nvl_task_state_t;
+/* Zero-copy plan of a task (tl_nvl_direct.c): where a post finds the members' buffers for its path's direct form - tables built
+ * from registrations at init, the tables the first post of a persistent request resolved, or the exchange board at every post.
+ * It holds no pointer into the task: nvl_rebuild swaps task bodies. */
+enum { NVL_ZC_SRC = 1, NVL_ZC_DST = 2, /* sides every member's direct form touches */
+       NVL_ZC_ALIGN = 4 /* a board entry that is not 16-byte aligned makes every member stage */ };
+typedef enum { NVL_ZC_RESOLVE, NVL_ZC_STAGED, NVL_ZC_DIRECT } nvl_zc_cache_t;
+typedef struct nvl_zc {
+    unsigned       flags;              /* NVL_ZC_*; 0: the direct form is not wanted */
+    const void    *src; void *dst; size_t src_len, dst_len; /* mine, as published */
+    nvl_zc_cache_t cache;              /* RESOLVE: at every post; STAGED / DIRECT: for every post, with the tables in d */
+    nvl_direct_t   d;
+    uint64_t       seq;                /* board entry of the current post */
+    int            published, pending; /* pending: the current post resolves through the board */
+} nvl_zc_t;
 typedef struct ucc_tl_nvl_task {
     ucc_coll_task_t     super;
     ucc_tl_nvl_team_t  *team;
@@ -211,15 +225,7 @@ typedef struct ucc_tl_nvl_task {
     /* zero-copy / deferred launch */
     nvl_task_state_t    state;
     ucc_list_link_t     q_elem;
-    int                 want_direct;   /* try the path's direct form for this collective */
-    int                 need_src, need_dst;
-    const void         *exp_src; void *exp_dst; size_t exp_src_len, exp_dst_len; /* what is published to the peers */
-    uint64_t            cseq;
-    int                 published;
-    int                 need_xchg;     /* this post goes through the buffer exchange (0: not zero-copy, or a persistent re-post whose tables are cached) */
-    int                 direct_cached; /* persistent request: the members' buffers were resolved by an earlier post (cached_mode / cached_d) */
-    int                 cached_mode;
-    nvl_direct_t        cached_d;
+    nvl_zc_t            zc;
     cudaEvent_t         in_event;
     /* send / recv */
     int                 p2p_rndv;      /* large message: rendezvous protocol */
@@ -250,11 +256,11 @@ ucc_status_t ucc_tl_nvl_xb_create(ucc_tl_nvl_team_t *team);
 ucc_status_t ucc_tl_nvl_xb_attach(ucc_tl_nvl_team_t *team);
 void         ucc_tl_nvl_xb_unlink(ucc_tl_nvl_team_t *team);
 void         ucc_tl_nvl_xb_release(ucc_tl_nvl_team_t *team);
-int          ucc_tl_nvl_xb_publish(ucc_tl_nvl_team_t *team, uint64_t cseq, const void *src, size_t src_len, void *dst, size_t dst_len, int usable, const size_t *aux);
 void         ucc_tl_nvl_xb_export(ucc_tl_nvl_team_t *team, const void *ptr, size_t len, nvl_xb_buf_t *b);
 char        *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b);
-int          ucc_tl_nvl_xb_ready(ucc_tl_nvl_team_t *team, uint64_t cseq);
-int          ucc_tl_nvl_xb_resolve(ucc_tl_nvl_team_t *team, uint64_t cseq, int need_src, int need_dst, int need_align, const void *my_src, void *my_dst, nvl_direct_t *d, size_t *aux_for_me);
+void         ucc_tl_nvl_zc_init(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, unsigned flags, const void *src, size_t src_len, void *dst, size_t dst_len, const ucc_coll_args_t *reg);
+void         ucc_tl_nvl_zc_post(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int captured, const size_t *aux);
+ucc_status_t ucc_tl_nvl_zc_ready(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int persistent, const size_t *aux, size_t *aux_for_me, int *direct);
 
 #define NVL_CTX(_team) ucc_derived_of((_team)->super.super.context, ucc_tl_nvl_context_t)
 extern ucc_tl_iface_t ucc_tl_nvl;

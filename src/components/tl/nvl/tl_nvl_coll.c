@@ -198,66 +198,18 @@ static void task_set_lane(ucc_tl_nvl_task_t *t, unsigned lane)
     d->mc_heap = team->dev.mc_heap ? team->dev.mc_heap + off : NULL;
 }
 
-/* every member published its buffers for this collective: pick (identically everywhere) the in-place kernel or
- * the staged one and fill the pointer tables */
-static ucc_status_t resolve_direct(ucc_tl_nvl_task_t *t)
+/* the one writer of the direct-form bit and tables: what the task's zero-copy plan resolved for this post (UCC_INPROGRESS: the
+ * members' buffers are not all known yet) */
+static ucc_status_t task_set_direct(ucc_tl_nvl_task_t *t)
 {
-    nvl_direct_t d;
-    int ok = ucc_tl_nvl_xb_resolve(t->team, t->cseq, t->need_src, t->need_dst, !path_uses_xchg(t->path), t->exp_src, t->exp_dst, &d, path_is_push(t->path) ? t->push.peer_land : NULL);
-    tl_debug(NVL_LIB(t->team), "exchange %lu: %s (src %d dst %d)", (unsigned long)t->cseq, ok > 0 ? "zero-copy" : (ok ? "MAPPING FAILED" : "staged"), t->need_src, t->need_dst);
-    if (ok < 0) {
-        tl_error(NVL_LIB(t->team), "cannot map a peer's buffer for the zero-copy kernel (the peers will run it): failing the collective; "
-                 "UCC_TL_NVL_ZCOPY=n avoids the zero-copy path");
-        return UCC_ERR_NO_RESOURCE;
-    }
-    if (path_uses_xchg(t->path)) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = d; }
-    else { t->u.red.direct = ok ? NVL_DIRECT_FULL : NVL_DIRECT_NONE; if (ok) t->u.red.d = d; }
-    /* persistent request: the buffers are fixed for the lifetime of the request, so every later post of it (same decision on
-     * every member - they all re-post the same request) launches straight away with these tables: no handle export, no board
-     * round trip, no deferred launch */
-    if (UCC_IS_PERSISTENT(t->super.bargs.args)) { t->direct_cached = 1; t->cached_mode = ok ? 1 : 0; t->cached_d = d; }
+    int push = path_is_push(t->path), direct;
+    ucc_status_t st;
+    if (!t->zc.flags) return UCC_OK;
+    st = ucc_tl_nvl_zc_ready(t->team, &t->zc, UCC_IS_PERSISTENT(t->super.bargs.args), push ? t->push.recv_off : NULL, push ? t->push.peer_land : NULL, &direct);
+    if (st != UCC_OK) return st;
+    if (path_uses_xchg(t->path)) { t->u.xchg.direct = direct; if (direct) t->u.xchg.d = t->zc.d; }
+    else { t->u.red.direct = direct ? NVL_DIRECT_FULL : NVL_DIRECT_NONE; if (direct) t->u.red.d = t->zc.d; }
     return UCC_OK;
-}
-static void apply_cached_direct(ucc_tl_nvl_task_t *t)
-{
-    int ok = t->cached_mode;
-    if (path_uses_xchg(t->path)) { t->u.xchg.direct = ok; if (ok) t->u.xchg.d = t->cached_d; }
-    else { t->u.red.direct = ok ? NVL_DIRECT_FULL : NVL_DIRECT_NONE; if (ok) t->u.red.d = t->cached_d; }
-}
-static inline int task_is_direct(const ucc_tl_nvl_task_t *t) { return t->want_direct && (t->team->zcopy || t->direct_cached); }
-
-/* Registered buffers: when the collective carries GLOBAL memory handles (one imported ucc_mem_map handle per member) for every
- * side the zero-copy kernel touches, the pointer tables are built right here from the registrations - the per-post exchange is
- * never used for this request.  Every member evaluates the same handles, flags and sizes, so the outcome is the same everywhere;
- * a member that cannot reach some segment could break that symmetry, so reachability of ALL segments is required on import
- * (unreachable -> h->mapped == NULL -> no table, and since the exporter could not produce an IPC handle either, nobody has one). */
-static void memh_direct(ucc_tl_nvl_task_t *t, const ucc_coll_args_t *a, const void *my_src, void *my_dst)
-{
-    ucc_tl_nvl_team_t *team = t->team;
-    const ucc_base_context_t *bctx = team->super.super.context;
-    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    int use_src = t->need_src && (a->mask & UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH) && (a->flags & UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL) && a->src_memh.global_memh;
-    int use_dst = t->need_dst && (a->mask & UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH) && (a->flags & UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL) && a->dst_memh.global_memh;
-    nvl_direct_t d;
-    if (!t->want_direct || (t->need_src && !use_src) || (t->need_dst && !use_dst)) return;
-    memset(&d, 0, sizeof(d));
-    for (int side = 0; side < 2; side++) {
-        ucc_mem_map_mem_h *gl = side ? a->dst_memh.global_memh : a->src_memh.global_memh;
-        const char *mine = side ? (const char *)my_dst : (const char *)my_src;
-        nvl_memh_t *hm;
-        size_t off;
-        if (side ? !use_dst : !use_src) continue;
-        hm = (nvl_memh_t *)ucc_mem_map_tl_handle(gl[me], bctx);
-        if (!hm || !hm->mapped || mine < hm->mapped || mine >= hm->mapped + hm->len) return; /* my buffer is not inside my registered segment */
-        off = (size_t)(mine - hm->mapped);
-        if ((uintptr_t)mine & 15) return;
-        for (ucc_rank_t p = 0; p < N; p++) {
-            nvl_memh_t *h = (nvl_memh_t *)ucc_mem_map_tl_handle(gl[p], bctx);
-            if (!h || !h->mapped || off >= h->len || ((uintptr_t)(h->mapped + off) & 15)) return;
-            if (side) d.dst[p] = p == me ? (char *)my_dst : h->mapped + off; else d.src[p] = p == me ? (const char *)my_src : h->mapped + off;
-        }
-    }
-    t->direct_cached = 1; t->cached_mode = 1; t->cached_d = d;
 }
 
 /* ------------------------------------------------------------------ */
@@ -401,28 +353,26 @@ static ucc_status_t p2p_post(ucc_tl_nvl_task_t *t, cudaStream_t s)
     return UCC_OK;
 }
 
+/* stream-ordered post: tell the consumer that the collective is in its stream now */
+static void ee_post_event(ucc_coll_task_t *ct)
+{
+    ucc_ev_t post_event;
+    post_event.ev_type = UCC_EVENT_COLLECTIVE_POST; post_event.ev_context = NULL; post_event.ev_context_size = 0; post_event.req = &ct->super;
+    ucc_ee_set_event_internal(ct->ee, &post_event, &ct->ee->event_out_queue);
+}
+
 /* head of the launch queue: start it once its buffer exchange (if any) is complete */
 static ucc_status_t try_launch_queued(ucc_tl_nvl_task_t *t)
 {
-    ucc_tl_nvl_team_t *team = t->team;
-    cudaStream_t s;
     ucc_status_t st;
-    if (ucc_list_head(&team->launch_q, ucc_tl_nvl_task_t, q_elem) != t) return UCC_INPROGRESS;
-    if (t->need_xchg) {
-        if (!t->published) t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, 1, path_is_push(t->path) ? t->push.recv_off : NULL);
-        if (!t->published || !ucc_tl_nvl_xb_ready(team, t->cseq)) return UCC_INPROGRESS;
-        st = resolve_direct(t);
-        if (st != UCC_OK) { ucc_list_del(&t->q_elem); t->state = NVL_TASK_LAUNCHED; return st; }
-    }
-    s = t->stream;
-    st = launch_ordered(t, s);
+    if (ucc_list_head(&t->team->launch_q, ucc_tl_nvl_task_t, q_elem) != t) return UCC_INPROGRESS;
+    st = task_set_direct(t);
+    if (st == UCC_INPROGRESS) return st;
+    if (st != UCC_OK) { ucc_list_del(&t->q_elem); t->state = NVL_TASK_LAUNCHED; return st; }
+    st = launch_ordered(t, t->stream);
     if (st != UCC_OK) return st;
     ucc_list_del(&t->q_elem); t->state = NVL_TASK_LAUNCHED;
-    if (t->super.ee) { /* stream-ordered post: only now is the collective really in the user's stream */
-        ucc_ev_t post_event;
-        post_event.ev_type = UCC_EVENT_COLLECTIVE_POST; post_event.ev_context = NULL; post_event.ev_context_size = 0; post_event.req = &t->super.super;
-        ucc_ee_set_event_internal(t->super.ee, &post_event, &t->super.ee->event_out_queue);
-    }
+    if (t->super.ee) ee_post_event(&t->super); /* only now is the collective really in the user's stream */
     return UCC_OK;
 }
 
@@ -446,10 +396,8 @@ static void nvl_progress(ucc_coll_task_t *ct)
         /* stream-ordered post: a send is in the user's stream once launched; a receive counts as posted once its buffer is on
          * the board (until then the owner has to keep progressing, nobody else can publish it) */
         if (t->state == NVL_TASK_LAUNCHED && !t->rz_pub_pending && !t->rz_wait_pending && t->super.ee && !t->p2p_ee_done) {
-            ucc_ev_t post_event;
             t->p2p_ee_done = 1;
-            post_event.ev_type = UCC_EVENT_COLLECTIVE_POST; post_event.ev_context = NULL; post_event.ev_context_size = 0; post_event.req = &t->super.super;
-            ucc_ee_set_event_internal(t->super.ee, &post_event, &t->super.ee->event_out_queue);
+            ee_post_event(ct);
         }
     }
     if (t->path == NVL_PATH_P2P && t->rz_wait_pending) return;   /* its event is not recorded yet */
@@ -497,9 +445,8 @@ static ucc_status_t nvl_post_on(ucc_tl_nvl_task_t *t, cudaStream_t s)
     ucc_status_t st;
     UCC_PROFILE_REQUEST_EVENT(t, "nvl_coll_start", 0);
     ucc_tl_nvl_team_t *team = t->team;
-    int direct;
     if (ucc_unlikely(t->super.flags & UCC_COLL_TASK_FLAG_ARGS_UPDATED)) { st = nvl_rebuild(t); if (st != UCC_OK) return st; }
-    t->stream = s; t->captured = 0; t->state = NVL_TASK_LAUNCHED; t->published = 0;
+    t->stream = s; t->captured = 0; t->state = NVL_TASK_LAUNCHED;
     if (cudaStreamIsCapturing(s, &cs) == cudaSuccess && cs == cudaStreamCaptureStatusActive) t->captured = 1;
     ucc_spin_lock(&team->launch_lock);
     /* lanes advance in post order, which UCC requires to be the same on every member; point-to-point and single-member tasks
@@ -512,24 +459,14 @@ static ucc_status_t nvl_post_on(ucc_tl_nvl_task_t *t, cudaStream_t s)
         return ucc_progress_queue_enqueue(UCC_TL_CORE_CTX(t->team)->pq, &t->super);
     }
     if (t->path != NVL_PATH_SELF_COPY && t->path != NVL_PATH_SELF_COPY_CE) task_set_lane(t, team->lane_seq++ % team->nlanes);
-    direct = task_is_direct(t) && !t->direct_cached;   /* cached tables: also fine inside a stream capture, nothing to wait for */
-    t->need_xchg = direct;
-    if (path_uses_xchg(t->path)) t->u.xchg.direct = 0; else t->u.red.direct = NVL_DIRECT_NONE;
-    if (task_is_direct(t) && t->direct_cached) apply_cached_direct(t);
-    if (direct) {
-        /* the exchange sequence advances on every rank in post order; a capturing stream cannot wait for the
-         * peers, so it tells them "not usable" and everybody takes the staged kernel for this one */
-        t->cseq = team->xb_seq++;
-        t->published = ucc_tl_nvl_xb_publish(team, t->cseq, t->exp_src, t->exp_src_len, t->exp_dst, t->exp_dst_len, !t->captured, path_is_push(t->path) ? t->push.recv_off : NULL);
-        if (t->captured) { direct = 0; t->need_xchg = 0; if (team->xb_mine->consumed < t->cseq + 1) ucc_store_release(&team->xb_mine->consumed, t->cseq + 1); }
-    }
-    if (t->captured || (ucc_list_is_empty(&team->launch_q) && (!direct || (t->published && ucc_tl_nvl_xb_ready(team, t->cseq))))) {
-        st = direct ? resolve_direct(t) : UCC_OK;
-        if (st == UCC_OK) st = launch_ordered(t, s);
-    } else {
+    if (t->zc.flags) ucc_tl_nvl_zc_post(team, &t->zc, t->captured, path_is_push(t->path) ? t->push.recv_off : NULL);
+    /* a captured post never waits: it has cached tables or runs staged */
+    st = t->captured || ucc_list_is_empty(&team->launch_q) ? task_set_direct(t) : UCC_INPROGRESS;
+    if (st == UCC_OK) st = launch_ordered(t, s);
+    else if (st == UCC_INPROGRESS) {
         /* deferred: the kernel is launched (into the same stream) from progress once the peers' buffers are known and
          * the tasks ahead of it are launched.  As with the reference's triggered post, a stream-ordered consumer
-         * learns from UCC_EVENT_COLLECTIVE_POST when the collective is really in its stream.  (Parking the user's
+         * learns from the post event (ee_post_event) when the collective is really in its stream.  (Parking the user's
          * stream on a cuStreamWaitValue32 gate was tried and dropped: streams share hardware channels, so the
          * parked wait can block the very kernel that is supposed to release it.) */
         st = UCC_OK;
@@ -547,7 +484,6 @@ static ucc_status_t nvl_post(ucc_coll_task_t *ct)
 static ucc_status_t nvl_triggered_post(ucc_ee_h ee, ucc_ev_t *ev, ucc_coll_task_t *ct)
 {
     ucc_tl_nvl_task_t *t = ucc_derived_of(ct, ucc_tl_nvl_task_t);
-    ucc_ev_t post_event;
     ucc_status_t st;
     (void)ev;
     if (ee->ee_type != UCC_EE_CUDA_STREAM) return UCC_ERR_NOT_SUPPORTED;
@@ -556,8 +492,7 @@ static ucc_status_t nvl_triggered_post(ucc_ee_h ee, ucc_ev_t *ev, ucc_coll_task_
     if (st != UCC_OK) return st;
     if (t->state == NVL_TASK_QUEUED || t->state == NVL_TASK_P2P_WAIT || (t->path == NVL_PATH_P2P && (t->rz_pub_pending || t->rz_wait_pending))) return UCC_OK; /* the post event follows the deferred launch / publication */
     t->p2p_ee_done = 1;
-    post_event.ev_type = UCC_EVENT_COLLECTIVE_POST; post_event.ev_context = NULL; post_event.ev_context_size = 0; post_event.req = &ct->super;
-    ucc_ee_set_event_internal(ee, &post_event, &ee->event_out_queue);
+    ee_post_event(ct);
     return UCC_OK;
 }
 static void event_put(ucc_tl_nvl_context_t *ctx, cudaEvent_t e);
@@ -607,8 +542,7 @@ static ucc_status_t task_alloc(ucc_base_coll_args_t *b, ucc_base_team_t *b_team,
     ucc_tl_nvl_task_t *t = (ucc_tl_nvl_task_t *)ucc_mpool_get(&ctx->task_mp);
     if (!t) return UCC_ERR_NO_MEMORY;
     ucc_coll_task_init(&t->super, b, b_team);
-    t->team = team; t->path = path; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->want_direct = 0;
-    t->need_xchg = 0; t->direct_cached = 0; t->cached_mode = 0; t->need_src = t->need_dst = 0; t->exp_src = NULL; t->exp_dst = NULL; t->exp_src_len = t->exp_dst_len = 0;
+    t->team = team; t->path = path; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->zc.flags = 0;
     t->nthreads = (int)ctx->cfg.nthreads;
     t->super.post = nvl_post; t->super.progress = nvl_progress; t->super.finalize = nvl_finalize; t->super.triggered_post = nvl_triggered_post;
     t->event = event_get(ctx);
@@ -709,7 +643,7 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
     nvl_path_t path;
     ucc_datatype_t dt; ucc_memory_type_t smt, dmt;
     const void *src; void *dst; size_t count, bytes;
-    int ndt, nop, nb, want_direct;
+    int ndt, nop, nb;
     ucc_status_t st;
     if (team->self) return self_init(b, b_team, task_p);
     switch (a->coll_type) {
@@ -796,19 +730,13 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
      * Every criterion below is evaluated identically on all ranks (sizes / counts are collective arguments); what only the owner
      * knows (can the buffer be exported? is it aligned?) travels with the exchange.  The NVLS kernels stay staged: writing the
      * result to N mapped destinations (NVL_DIRECT_DST) instead of one multicast store multiplies the bytes leaving each GPU by
-     * 1.75 on 8 members */
-    want_direct = path == NVL_PATH_TWOSHOT && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh &&
-                  (team->zcopy || (a->mask & (UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH))) &&
-                  (r.kind != NVL_RED_REDUCE_SCATTER || rs_offsets_aligned(&r, dt));
+     * 1.75 on 8 members.  Reduce_scatter maps the sources only, reduce uses no registrations. */
     st = task_alloc(b, b_team, path, &t);
     if (st != UCC_OK) return st;
     t->u.red = r; t->nblocks = nb;
-    if (want_direct) {
-        t->want_direct = 1; t->need_src = 1; t->need_dst = r.kind != NVL_RED_REDUCE_SCATTER;
-        t->exp_src = src; t->exp_src_len = bytes;
-        t->exp_dst = r.kind == NVL_RED_REDUCE_SCATTER ? NULL : dst; t->exp_dst_len = t->exp_dst ? bytes : 0;
-        if (r.kind != NVL_RED_REDUCE) memh_direct(t, a, src, dst);
-        if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
+    if (path == NVL_PATH_TWOSHOT && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh && (r.kind != NVL_RED_REDUCE_SCATTER || rs_offsets_aligned(&r, dt))) {
+        int rs = r.kind == NVL_RED_REDUCE_SCATTER;
+        ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_SRC | NVL_ZC_ALIGN | (rs ? 0 : NVL_ZC_DST), src, bytes, rs ? NULL : dst, bytes, r.kind != NVL_RED_REDUCE ? a : NULL);
     }
     *task_p = &t->super;
     return UCC_OK;
@@ -1003,18 +931,13 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     if (path == NVL_PATH_SWAP && ctx->cfg.zcopy != UCC_NO && (size_t)nb * NVL_SWAP_TABLE_BYTES <= ctx->cfg.symmetric_size) {
         /* the buffers travel over the exchange board (or come from registrations) as destinations: the swap kernel reads and
          * writes them in place, and when they do not resolve, launch_swap stages */
-        t->want_direct = 1; t->need_dst = 1;
-        t->exp_dst = x.dst; t->exp_dst_len = x.src_bytes;
-        memh_direct(t, a, NULL, x.dst);
-        if (!t->direct_cached && !team->zcopy) t->want_direct = 0;
+        ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, x.dst, x.src_bytes, a);
     }
     /* (private sizes: always - the choice may only depend on what every rank knows, and staging a skewed alltoallv through the
      * heap was 2.4x slower than NCCL at 16 MB on 4 GPUs; below ~4 MB the host-side exchange costs more than the staging copy) */
     if (path == NVL_PATH_PULL && team->zcopy && ctx->cfg.zcopy != UCC_NO &&
-        (private_sizes || moved >= (ctx->cfg.zcopy == UCC_YES ? ctx->cfg.zcopy_thresh : ucc_max(ctx->cfg.zcopy_thresh, (size_t)4 << 20)))) {
-        t->want_direct = 1; t->need_src = 1;
-        t->exp_src = x.src_bytes ? x.src : NULL; t->exp_src_len = x.src_bytes;
-    }
+        (private_sizes || moved >= (ctx->cfg.zcopy == UCC_YES ? ctx->cfg.zcopy_thresh : ucc_max(ctx->cfg.zcopy_thresh, (size_t)4 << 20))))
+        ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_SRC, x.src_bytes ? x.src : NULL, x.src_bytes, NULL, 0, NULL);
     if (path_is_push(path)) {
         /* the destinations travel over the exchange board and every rank stores its blocks straight into them; if a destination
          * cannot be mapped the task runs the staged pull */
@@ -1031,8 +954,7 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
             else { t->push.send_off[p] = 0; t->push.send_bytes[p] = x.pull_bytes[me]; t->push.land_off[p] = x.dst_off[me]; } /* my block, at my displacement, in everybody's dst */
             if (x.dst_off[p] + x.pull_bytes[p] > dst_len) dst_len = x.dst_off[p] + x.pull_bytes[p];
         }
-        t->want_direct = 1; t->need_dst = 1;
-        t->exp_dst = x.dst; t->exp_dst_len = dst_len;
+        ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, x.dst, dst_len, NULL);
     }
     *task_p = &t->super;
     return UCC_OK;

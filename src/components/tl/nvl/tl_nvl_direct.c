@@ -80,23 +80,16 @@ static void export_buf(ucc_tl_nvl_team_t *team, const void *ptr, size_t len, nvl
 void ucc_tl_nvl_xb_export(ucc_tl_nvl_team_t *team, const void *ptr, size_t len, nvl_xb_buf_t *b) { export_buf(team, ptr, len, b); }
 
 /* returns 0 when the slot is still in use by a slow peer (caller retries later) */
-int ucc_tl_nvl_xb_publish(ucc_tl_nvl_team_t *team, uint64_t cseq, const void *src, size_t src_len, void *dst, size_t dst_len, int usable, const size_t *aux)
+static int xb_publish(ucc_tl_nvl_team_t *team, const nvl_zc_t *zc, int usable, const size_t *aux)
 {
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    nvl_xb_entry_t *e = &team->xb_mine->e[cseq % NVL_XB_SLOTS];
-    if (cseq >= NVL_XB_SLOTS)
-        for (ucc_rank_t p = 0; p < N; p++) if (p != me && ucc_load_acquire(&team->xb[p]->consumed) + NVL_XB_SLOTS <= cseq) return 0;
-    if (usable) { export_buf(team, src, src_len, &e->src); export_buf(team, dst, dst_len, &e->dst); }
+    nvl_xb_entry_t *e = &team->xb_mine->e[zc->seq % NVL_XB_SLOTS];
+    if (zc->seq >= NVL_XB_SLOTS)
+        for (ucc_rank_t p = 0; p < N; p++) if (p != me && ucc_load_acquire(&team->xb[p]->consumed) + NVL_XB_SLOTS <= zc->seq) return 0;
+    if (usable) { export_buf(team, zc->src, zc->src_len, &e->src); export_buf(team, zc->dst, zc->dst_len, &e->dst); }
     else { memset(&e->src, 0, sizeof(e->src)); memset(&e->dst, 0, sizeof(e->dst)); e->src.kind = e->dst.kind = NVL_XB_NONE; }
     for (ucc_rank_t p = 0; p < N && p < NVL_MAX_PEERS; p++) e->aux[p] = aux ? (uint64_t)aux[p] : 0;
-    ucc_store_release(&e->seq, cseq + 1);
-    return 1;
-}
-
-int ucc_tl_nvl_xb_ready(ucc_tl_nvl_team_t *team, uint64_t cseq)
-{
-    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    for (ucc_rank_t p = 0; p < N; p++) if (p != me && ucc_load_acquire(&team->xb[p]->e[cseq % NVL_XB_SLOTS].seq) != cseq + 1) return 0;
+    ucc_store_release(&e->seq, zc->seq + 1);
     return 1;
 }
 
@@ -130,17 +123,76 @@ static char *import_buf(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_
 
 char *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b) { return import_buf(team, p, b); }
 
-/* all members published: decide (identically on every rank) whether the buffers can be used in place and map
- * them.  need_src / need_dst say which sides the kernel touches remotely.  Marks the entries consumed.
- * Returns 1 = in place, 0 = every member stages (symmetric decision), -1 = local mapping failure (the collective must fail). */
-int ucc_tl_nvl_xb_resolve(ucc_tl_nvl_team_t *team, uint64_t cseq, int need_src, int need_dst, int need_align, const void *my_src, void *my_dst, nvl_direct_t *d, size_t *aux_for_me)
+/* Registered buffers: when the collective carries GLOBAL memory handles (one imported ucc_mem_map handle per member) for every
+ * side the zero-copy kernel touches, the pointer tables are built at init from the registrations - the per-post exchange is
+ * never used for this request.  Every member evaluates the same handles, flags and sizes, so the outcome is the same everywhere;
+ * a member that cannot reach some segment could break that symmetry, so reachability of ALL segments is required on import
+ * (unreachable -> h->mapped == NULL -> no table, and since the exporter could not produce an IPC handle either, nobody has one). */
+static int memh_tables(ucc_tl_nvl_team_t *team, const ucc_coll_args_t *a, nvl_zc_t *zc)
+{
+    const ucc_base_context_t *bctx = team->super.super.context;
+    ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
+    int need_src = zc->flags & NVL_ZC_SRC, need_dst = zc->flags & NVL_ZC_DST;
+    int use_src = need_src && (a->mask & UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH) && (a->flags & UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL) && a->src_memh.global_memh;
+    int use_dst = need_dst && (a->mask & UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH) && (a->flags & UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL) && a->dst_memh.global_memh;
+    if ((need_src && !use_src) || (need_dst && !use_dst)) return 0;
+    memset(&zc->d, 0, sizeof(zc->d));
+    for (int side = 0; side < 2; side++) {
+        ucc_mem_map_mem_h *gl = side ? a->dst_memh.global_memh : a->src_memh.global_memh;
+        const char *mine = side ? (const char *)zc->dst : (const char *)zc->src;
+        nvl_memh_t *hm;
+        size_t off;
+        if (side ? !use_dst : !use_src) continue;
+        hm = (nvl_memh_t *)ucc_mem_map_tl_handle(gl[me], bctx);
+        if (!hm || !hm->mapped || mine < hm->mapped || mine >= hm->mapped + hm->len) return 0; /* my buffer is not inside my registered segment */
+        off = (size_t)(mine - hm->mapped);
+        if ((uintptr_t)mine & 15) return 0;
+        for (ucc_rank_t p = 0; p < N; p++) {
+            nvl_memh_t *h = (nvl_memh_t *)ucc_mem_map_tl_handle(gl[p], bctx);
+            if (!h || !h->mapped || off >= h->len || ((uintptr_t)(h->mapped + off) & 15)) return 0;
+            if (side) zc->d.dst[p] = p == me ? (char *)zc->dst : h->mapped + off; else zc->d.src[p] = p == me ? (const char *)zc->src : h->mapped + off;
+        }
+    }
+    return 1;
+}
+
+/* at init: the plan of a task whose path has a direct form.  `flags`: NVL_ZC_*; src / dst: my buffers as the peers see them;
+ * `reg`: the arguments whose registrations may give the tables (NULL: never) */
+void ucc_tl_nvl_zc_init(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, unsigned flags, const void *src, size_t src_len, void *dst, size_t dst_len, const ucc_coll_args_t *reg)
+{
+    zc->flags = flags; zc->src = src; zc->src_len = src_len; zc->dst = dst; zc->dst_len = dst_len;
+    zc->cache = reg && memh_tables(team, reg, zc) ? NVL_ZC_DIRECT : NVL_ZC_RESOLVE;
+    if (zc->cache == NVL_ZC_RESOLVE && !team->zcopy) zc->flags = 0; /* no board and nothing cached: always staged */
+}
+
+/* at post, in post order (the same on every member): a post without a cached decision takes the next board entry and publishes
+ * my buffers (aux: what every member reads back at my index).  A capturing stream cannot wait for the peers, so it tells them
+ * "not usable" and everybody stages this one; cached tables need no waiting and are also fine inside a capture. */
+void ucc_tl_nvl_zc_post(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int captured, const size_t *aux)
+{
+    zc->pending = zc->cache == NVL_ZC_RESOLVE;
+    if (!zc->pending) return;
+    zc->seq = team->xb_seq++;
+    zc->published = xb_publish(team, zc, !captured, aux);
+    if (captured) { zc->pending = 0; if (team->xb_mine->consumed < zc->seq + 1) ucc_store_release(&team->xb_mine->consumed, zc->seq + 1); }
+}
+
+/* *direct: whether this post runs the direct form, with the tables in zc->d.  UCC_INPROGRESS: not every member has published
+ * yet (call again).  aux_for_me: what every member published at my index. */
+ucc_status_t ucc_tl_nvl_zc_ready(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int persistent, const size_t *aux, size_t *aux_for_me, int *direct)
 {
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
-    int ok = 1;
+    int need_src = zc->flags & NVL_ZC_SRC, need_dst = zc->flags & NVL_ZC_DST, need_align = zc->flags & NVL_ZC_ALIGN, ok = 1;
+    nvl_direct_t *d = &zc->d;
+    if (!zc->pending) { *direct = zc->cache == NVL_ZC_DIRECT; return UCC_OK; }
+    if (!zc->published) zc->published = xb_publish(team, zc, 1, aux);
+    if (!zc->published) return UCC_INPROGRESS;
+    for (ucc_rank_t p = 0; p < N; p++) if (p != me && ucc_load_acquire(&team->xb[p]->e[zc->seq % NVL_XB_SLOTS].seq) != zc->seq + 1) return UCC_INPROGRESS;
+    /* all members published: decide (identically on every rank) whether the buffers can be used in place and map them */
     memset(d, 0, sizeof(*d));
-    if (aux_for_me) for (ucc_rank_t p = 0; p < N; p++) aux_for_me[p] = (size_t)team->xb[p]->e[cseq % NVL_XB_SLOTS].aux[me];
+    if (aux_for_me) for (ucc_rank_t p = 0; p < N; p++) aux_for_me[p] = (size_t)team->xb[p]->e[zc->seq % NVL_XB_SLOTS].aux[me];
     for (ucc_rank_t p = 0; p < N && ok; p++) {
-        const nvl_xb_entry_t *e = &team->xb[p]->e[cseq % NVL_XB_SLOTS];
+        const nvl_xb_entry_t *e = &team->xb[p]->e[zc->seq % NVL_XB_SLOTS];
         if (need_src && e->src.kind != NVL_XB_EMPTY && e->src.kind != NVL_XB_RAW && e->src.kind != NVL_XB_IPC) ok = 0;
         if (need_dst && e->dst.kind != NVL_XB_EMPTY && e->dst.kind != NVL_XB_RAW && e->dst.kind != NVL_XB_IPC) ok = 0;
         /* 16-byte alignment keeps every transaction a full vector; anything else takes the staged kernel */
@@ -149,13 +201,26 @@ int ucc_tl_nvl_xb_resolve(ucc_tl_nvl_team_t *team, uint64_t cseq, int need_src, 
     }
     /* up to here every member took the same decision (it only depends on what all of them published).  Mapping a peer's
      * allocation can still fail on THIS rank only; the peers will launch the in-place kernel, so falling back to the staged
-     * one here would mix two protocols and corrupt data silently: report it (-1), the caller fails the collective. */
+     * one here would mix two protocols and corrupt data silently: fail the collective. */
     for (ucc_rank_t p = 0; p < N && ok > 0; p++) {
-        const nvl_xb_entry_t *e = &team->xb[p]->e[cseq % NVL_XB_SLOTS];
-        if (p == me) { d->src[p] = (const char *)my_src; d->dst[p] = (char *)my_dst; continue; }
+        const nvl_xb_entry_t *e = &team->xb[p]->e[zc->seq % NVL_XB_SLOTS];
+        if (p == me) { d->src[p] = (const char *)zc->src; d->dst[p] = (char *)zc->dst; continue; }
         if (need_src && e->src.kind != NVL_XB_EMPTY) { d->src[p] = import_buf(team, p, &e->src); if (!d->src[p]) ok = -1; }
         if (need_dst && e->dst.kind != NVL_XB_EMPTY) { d->dst[p] = import_buf(team, p, &e->dst); if (!d->dst[p]) ok = -1; }
     }
-    if (team->xb_mine->consumed < cseq + 1) ucc_store_release(&team->xb_mine->consumed, cseq + 1);
-    return ok;
+    if (team->xb_mine->consumed < zc->seq + 1) ucc_store_release(&team->xb_mine->consumed, zc->seq + 1);
+    tl_debug(NVL_LIB(team), "exchange %lu: %s (src %d dst %d)", (unsigned long)zc->seq, ok > 0 ? "zero-copy" : (ok ? "MAPPING FAILED" : "staged"),
+             !!need_src, !!need_dst);
+    if (ok < 0) {
+        tl_error(NVL_LIB(team), "cannot map a peer's buffer for the zero-copy kernel (the peers will run it): failing the collective; "
+                 "UCC_TL_NVL_ZCOPY=n avoids the zero-copy path");
+        return UCC_ERR_NO_RESOURCE;
+    }
+    zc->pending = 0;
+    /* persistent request: the buffers are fixed for the lifetime of the request, so every later post of it (same decision on
+     * every member - they all re-post the same request) launches straight away with these tables: no handle export, no board
+     * round trip, no deferred launch */
+    if (persistent) zc->cache = ok ? NVL_ZC_DIRECT : NVL_ZC_STAGED;
+    *direct = ok;
+    return UCC_OK;
 }

@@ -7,7 +7,7 @@
  *   IMPORT  open the allocation (cached per context by allocation base + handle bytes) -> a pointer valid here
  *
  * A collective whose arguments carry GLOBAL handles (UCC_COLL_ARGS_FLAG_{SRC,DST}_MEMH_GLOBAL: one imported handle per member)
- * gets its zero-copy pointer tables from them at init time (tl_nvl_coll.c: memh_direct): no per-post handle export, no exchange
+ * gets its zero-copy pointer tables from them at init time (tl_nvl_direct.c: ucc_tl_nvl_zc_init): no per-post handle export, no exchange
  * board round trip, no deferred launch - the registration is paid once.  Convention (same as the reference's one-sided
  * algorithms): a member's buffer sits at the same offset inside its registered segment on every member. */
 #include "tl_nvl.h"
