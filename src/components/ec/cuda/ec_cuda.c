@@ -160,6 +160,7 @@ static int to_ec_dt(ucc_datatype_t dt)
     case UCC_DT_UINT8: return EC_DT_U8; case UCC_DT_UINT16: return EC_DT_U16; case UCC_DT_UINT32: return EC_DT_U32; case UCC_DT_UINT64: return EC_DT_U64;
     case UCC_DT_FLOAT16: return EC_DT_F16; case UCC_DT_FLOAT32: return EC_DT_F32; case UCC_DT_FLOAT64: return EC_DT_F64; case UCC_DT_BFLOAT16: return EC_DT_BF16;
     case UCC_DT_FLOAT32_COMPLEX: return EC_DT_C64; case UCC_DT_FLOAT64_COMPLEX: return EC_DT_C128;
+    case UCC_DT_INT128: return EC_DT_I128; case UCC_DT_UINT128: return EC_DT_U128;
     default: return -1;
     }
 }

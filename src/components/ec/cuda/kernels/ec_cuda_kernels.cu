@@ -27,15 +27,15 @@ template <> __device__ __forceinline__ cuDoubleComplex scale(cuDoubleComplex x, 
 static __device__ __forceinline__ const void *src_k(const ec_reduce_args_t &a, int k)
 { return (!a.strided || k == 0) ? a.srcs[a.strided ? 0 : k] : (const char *)a.src2 + (size_t)(k - 1) * a.stride; }
 
-/* scalar path: any alignment, any type */
+/* scalar path: any alignment, any type (ld_elem / st_elem: a 128-bit integer may sit at an 8-byte aligned address) */
 template <typename T, typename A, int OP, typename LD, typename ST>
 static __device__ __forceinline__ void reduce_scalar(const ec_reduce_args_t &a, size_t begin, size_t end, LD ld, ST st, size_t tid, size_t nt)
 {
     for (size_t i = begin + tid; i < end; i += nt) {
-        A acc = ld(((const T *)src_k(a, 0))[i]);
-        for (int k = 1; k < a.n_srcs; k++) acc = EcOp<OP, A>::f(acc, ld(((const T *)src_k(a, k))[i]));
+        A acc = ld(ld_elem((const T *)src_k(a, 0) + i));
+        for (int k = 1; k < a.n_srcs; k++) acc = EcOp<OP, A>::f(acc, ld(ld_elem((const T *)src_k(a, k) + i)));
         if (a.with_alpha) acc = scale<A>(acc, a.alpha);
-        ((T *)a.dst)[i] = st(acc);
+        st_elem((T *)a.dst + i, st(acc));
     }
 }
 
@@ -78,6 +78,7 @@ static __device__ __noinline__ void reduce_any(const ec_reduce_args_t &a, size_t
     case EC_DT_U32: reduce_dispatch<uint32_t>(a, tid, nt); break; case EC_DT_U64: reduce_dispatch<uint64_t>(a, tid, nt); break;
     case EC_DT_F16: reduce_dispatch<__half>(a, tid, nt); break; case EC_DT_BF16: reduce_dispatch<__nv_bfloat16>(a, tid, nt); break;
     case EC_DT_F32: reduce_dispatch<float>(a, tid, nt); break; case EC_DT_F64: reduce_dispatch<double>(a, tid, nt); break;
+    case EC_DT_I128: reduce_dispatch<nvl_i128>(a, tid, nt); break; case EC_DT_U128: reduce_dispatch<nvl_u128>(a, tid, nt); break;
     case EC_DT_C64: if (a.op == EC_OP_SUM) reduce_body_cplx<cuFloatComplex, EC_OP_SUM>(a, tid, nt); else if (a.op == EC_OP_PROD) reduce_body_cplx<cuFloatComplex, EC_OP_PROD>(a, tid, nt); break;
     case EC_DT_C128: if (a.op == EC_OP_SUM) reduce_body_cplx<cuDoubleComplex, EC_OP_SUM>(a, tid, nt); else if (a.op == EC_OP_PROD) reduce_body_cplx<cuDoubleComplex, EC_OP_PROD>(a, tid, nt); break;
     default: break;
@@ -179,7 +180,7 @@ __global__ void ec_wait_kernel(volatile uint32_t *state) { while (*state == 0) {
 
 /* ------------------------------------------------------------------ */
 extern "C" size_t ec_dt_size(int dt)
-{ static const size_t s[EC_DT_LAST] = {1, 2, 4, 8, 1, 2, 4, 8, 2, 4, 8, 2, 8, 16}; return dt >= 0 && dt < EC_DT_LAST ? s[dt] : 0; }
+{ static const size_t s[EC_DT_LAST] = {1, 2, 4, 8, 1, 2, 4, 8, 2, 4, 8, 2, 8, 16, 16, 16}; return dt >= 0 && dt < EC_DT_LAST ? s[dt] : 0; }
 extern "C" int ec_dt_supports_op(int dt, int op)
 {
     if (dt < 0 || dt >= EC_DT_LAST || op < 0 || op >= EC_OP_LAST) return 0;
@@ -196,6 +197,7 @@ extern "C" cudaError_t ec_launch_reduce(const ec_reduce_args_t *a, int nblocks, 
     case EC_DT_U32: return ec_launch_reduce_t<uint32_t>(a, nblocks, nthreads, s); case EC_DT_U64: return ec_launch_reduce_t<uint64_t>(a, nblocks, nthreads, s);
     case EC_DT_F16: return ec_launch_reduce_t<__half>(a, nblocks, nthreads, s); case EC_DT_BF16: return ec_launch_reduce_t<__nv_bfloat16>(a, nblocks, nthreads, s);
     case EC_DT_F32: return ec_launch_reduce_t<float>(a, nblocks, nthreads, s); case EC_DT_F64: return ec_launch_reduce_t<double>(a, nblocks, nthreads, s);
+    case EC_DT_I128: return ec_launch_reduce_t<nvl_i128>(a, nblocks, nthreads, s); case EC_DT_U128: return ec_launch_reduce_t<nvl_u128>(a, nblocks, nthreads, s);
     case EC_DT_C64:
         if (a->op == EC_OP_SUM) ec_reduce_cplx_kernel_t<cuFloatComplex, EC_OP_SUM><<<nblocks, nthreads, 0, s>>>(*a);
         else if (a->op == EC_OP_PROD) ec_reduce_cplx_kernel_t<cuFloatComplex, EC_OP_PROD><<<nblocks, nthreads, 0, s>>>(*a);

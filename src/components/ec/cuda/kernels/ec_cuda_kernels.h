@@ -10,7 +10,7 @@
 #define EC_MAX_SRCS 16
 #define EC_MULTI_BUFS 7
 typedef enum { EC_DT_I8, EC_DT_I16, EC_DT_I32, EC_DT_I64, EC_DT_U8, EC_DT_U16, EC_DT_U32, EC_DT_U64, EC_DT_F16, EC_DT_F32, EC_DT_F64,
-               EC_DT_BF16, EC_DT_C64, EC_DT_C128, EC_DT_LAST } ec_dt_t;
+               EC_DT_BF16, EC_DT_C64, EC_DT_C128, EC_DT_I128, EC_DT_U128, EC_DT_LAST } ec_dt_t;
 typedef enum { EC_OP_SUM, EC_OP_PROD, EC_OP_MAX, EC_OP_MIN, EC_OP_LAND, EC_OP_LOR, EC_OP_LXOR, EC_OP_BAND, EC_OP_BOR, EC_OP_BXOR, EC_OP_LAST } ec_op_t;
 typedef enum { EC_TASK_NONE, EC_TASK_REDUCE, EC_TASK_REDUCE_MULTI_DST, EC_TASK_COPY, EC_TASK_COPY_MULTI } ec_task_kind_t;
 

@@ -135,13 +135,35 @@ struct BlockSync {
 /* ------------------------------------------------------------------ */
 template <typename T> struct Vec { static constexpr int E = 16 / sizeof(T); union { uint4 v; T e[16 / sizeof(T)]; }; };
 
+/* 128-bit integers (UCC_DT_INT128 / UINT128): one element per 16-byte vector.  Each is its own accumulator, so sums and
+ * products wrap mod 2^128; MAX / MIN compare signed resp. unsigned. */
+typedef __int128 nvl_i128;
+typedef unsigned __int128 nvl_u128;
+static_assert(sizeof(nvl_i128) == 16 && alignof(nvl_i128) == 16 && alignof(nvl_u128) == 16, "128-bit integers fill one 16-byte vector");
+template <typename T> struct IsInt128 { static constexpr bool v = false; };
+template <> struct IsInt128<nvl_i128> { static constexpr bool v = true; };
+template <> struct IsInt128<nvl_u128> { static constexpr bool v = true; };
+
+/* one element of the guarded path.  A 128-bit integer there may sit at an address that is only 8-byte aligned (the reason the
+ * vector path was not taken), where a 16-byte access faults: it moves as two 8-byte words */
+template <typename T> NVL_DEV T ld_elem(const T *p)
+{
+    if constexpr (IsInt128<T>::v) { const uint64_t *w = reinterpret_cast<const uint64_t *>(p); return (T)((nvl_u128)w[1] << 64 | w[0]); }
+    else return *p;
+}
+template <typename T> NVL_DEV void st_elem(T *p, T x)
+{
+    if constexpr (IsInt128<T>::v) { uint64_t *w = reinterpret_cast<uint64_t *>(p); w[0] = (uint64_t)x; w[1] = (uint64_t)((nvl_u128)x >> 64); }
+    else *p = x;
+}
+
 template <typename T> NVL_DEV uint4 load_src_vec(const T *base, size_t idx, size_t n, bool aligned)
 {
     constexpr int E = 16 / sizeof(T);
     if (aligned && idx + E <= n) return ld_src_v4(base + idx);
     Vec<T> u; u.v = make_uint4(0, 0, 0, 0);
 #pragma unroll
-    for (int i = 0; i < E; i++) if (idx + i < n) u.e[i] = base[idx + i];
+    for (int i = 0; i < E; i++) if (idx + i < n) u.e[i] = ld_elem(base + idx + i);
     return u.v;
 }
 template <typename T> NVL_DEV void store_dst_vec(T *base, size_t idx, size_t n, bool aligned, uint4 x)
@@ -150,7 +172,7 @@ template <typename T> NVL_DEV void store_dst_vec(T *base, size_t idx, size_t n, 
     if (aligned && idx + E <= n) { st_v4(base + idx, x); return; }
     Vec<T> u; u.v = x;
 #pragma unroll
-    for (int i = 0; i < E; i++) if (idx + i < n) base[idx + i] = u.e[i];
+    for (int i = 0; i < E; i++) if (idx + i < n) st_elem(base + idx + i, u.e[i]);
 }
 
 /* ------------------------------------------------------------------ */
@@ -205,10 +227,27 @@ template <typename R> NVL_DEV R inv_n_as(float inv_n, int n)
     if constexpr (sizeof(R) == sizeof(double)) return 1.0 / (double)n;
     else return (R)inv_n;
 }
+/* x / n, truncating, for a 128-bit integer and a team size n: long division in 64-by-32-bit steps.  The general 128-bit division
+ * the compiler emits for x / (A)n is a call whose frame spills to the local-memory stack in the zero-copy kernel. */
+NVL_DEV nvl_u128 udiv128_by_small(nvl_u128 x, uint32_t n)
+{
+    const uint64_t hi = (uint64_t)(x >> 64), lo = (uint64_t)x;
+    const uint64_t qh = hi / n;
+    uint64_t t = (hi % n) << 32 | lo >> 32;     /* remainder < n < 2^32: every partial quotient below fits 32 bits */
+    const uint64_t q1 = t / n;
+    t = (t % n) << 32 | (lo & 0xffffffffu);
+    return (nvl_u128)qh << 64 | (nvl_u128)(q1 << 32 | t / n);
+}
+template <typename A> NVL_DEV A div128_by_small(A x, int n)
+{
+    if constexpr ((A)-1 > (A)0) return udiv128_by_small(x, (uint32_t)n);
+    else return x < 0 ? -(A)udiv128_by_small(-(nvl_u128)x, (uint32_t)n) : (A)udiv128_by_small((nvl_u128)x, (uint32_t)n);
+}
 template <int OP, typename A> NVL_DEV A avg_scale(A x, float inv_n, int n)
 {
     if (OP != NVL_OP_AVG) return x;
-    if constexpr (IsIntAcc<A>::v) return n > 1 ? (A)(x / (A)n) : x;
+    if constexpr (IsInt128<A>::v) return n > 1 ? div128_by_small(x, n) : x;
+    else if constexpr (IsIntAcc<A>::v) return n > 1 ? (A)(x / (A)n) : x;
     else if constexpr (IsComplex<A>::v) { const auto s = inv_n_as<decltype(x.re)>(inv_n, n); return {x.re * s, x.im * s}; } /* as the real type */
     else return x * inv_n_as<A>(inv_n, n);
 }

@@ -212,11 +212,11 @@ __global__ void __launch_bounds__(NVL_THREADS_MAX, 2) nvl_exchange_kernel(nvl_xc
 /* host-side launchers                                                 */
 /* ------------------------------------------------------------------ */
 #ifndef NVL_HOST_EMU /* tests/emu includes the kernels above and calls them directly */
-/* the rows of the reduction kernels in nvl_dt_t order, each defined by its nvl_red_<dt>.cu */
+/* the rows of the reduction kernels in nvl_dt_t order, each defined by its nvl_red_<dt>.cu (float128 has none) */
 extern const nvl_dt_row nvl_row_i8, nvl_row_i16, nvl_row_i32, nvl_row_i64, nvl_row_u8, nvl_row_u16, nvl_row_u32, nvl_row_u64, nvl_row_f16, nvl_row_f32,
-    nvl_row_f64, nvl_row_bf16, nvl_row_c64, nvl_row_c128;
+    nvl_row_f64, nvl_row_bf16, nvl_row_c64, nvl_row_c128, nvl_row_i128, nvl_row_u128;
 static const nvl_dt_row *const nvl_rows[NVL_DT_LAST] = {&nvl_row_i8, &nvl_row_i16, &nvl_row_i32, &nvl_row_i64, &nvl_row_u8, &nvl_row_u16, &nvl_row_u32,
-    &nvl_row_u64, &nvl_row_f16, &nvl_row_f32, &nvl_row_f64, &nvl_row_bf16, &nvl_row_c64, &nvl_row_c128};
+    &nvl_row_u64, &nvl_row_f16, &nvl_row_f32, &nvl_row_f64, &nvl_row_bf16, &nvl_row_c64, &nvl_row_c128, nullptr, &nvl_row_i128, &nvl_row_u128};
 static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nblocks, int nthreads, cudaStream_t s)
 {
     k<<<nblocks, nthreads, 0, s>>>(a);

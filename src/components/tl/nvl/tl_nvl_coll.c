@@ -18,6 +18,7 @@ static int to_nvl_dt(ucc_datatype_t dt)
     case UCC_DT_UINT8: return NVL_DT_U8; case UCC_DT_UINT16: return NVL_DT_U16; case UCC_DT_UINT32: return NVL_DT_U32; case UCC_DT_UINT64: return NVL_DT_U64;
     case UCC_DT_FLOAT16: return NVL_DT_F16; case UCC_DT_FLOAT32: return NVL_DT_F32; case UCC_DT_FLOAT64: return NVL_DT_F64; case UCC_DT_BFLOAT16: return NVL_DT_BF16;
     case UCC_DT_FLOAT32_COMPLEX: return NVL_DT_C64; case UCC_DT_FLOAT64_COMPLEX: return NVL_DT_C128;
+    case UCC_DT_INT128: return NVL_DT_I128; case UCC_DT_UINT128: return NVL_DT_U128; case UCC_DT_FLOAT128: return NVL_DT_F128;
     default: return -1;
     }
 }

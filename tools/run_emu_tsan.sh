@@ -6,8 +6,9 @@ set -e
 cd "$(dirname "$0")/.."
 K=src/components/tl/nvl/kernels
 rc=0
-# driver:modes (the complex and swap drivers run everything in one mode)
-for spec in "nvl_emu:staged xchg pipe symm push oneshot_rs soak soak2" "nvl_emu_complex:complex" "nvl_emu_swap:swap"; do
+# driver:modes (the complex, swap and int128 drivers run everything in one mode); arguments: the drivers to run (default: all)
+for spec in "nvl_emu:staged xchg pipe symm push oneshot_rs soak soak2" "nvl_emu_complex:complex" "nvl_emu_swap:swap" "nvl_emu_int128:int128"; do
+  if [ $# -gt 0 ] && [[ " $* " != *" ${spec%%:*} "* ]]; then continue; fi
   exe=/tmp/ucc_b200_${spec%%:*}_tsan
   /usr/bin/g++ -O1 -g -fsanitize=thread -std=c++17 -pthread -I/usr/local/cuda/include -I$K -Iinclude -Isrc tests/emu/${spec%%:*}.cpp -o $exe
   for w in ${spec#*:}; do
