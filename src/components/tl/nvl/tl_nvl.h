@@ -69,7 +69,12 @@ typedef struct nvl_xb_entry { uint64_t seq; nvl_xb_buf_t src, dst; uint64_t aux[
 typedef struct nvl_xb_rz { uint64_t seq; nvl_xb_buf_t buf; } nvl_xb_rz_t;
 typedef struct nvl_xb_seg { uint64_t consumed; uint64_t pad[7]; nvl_xb_entry_t e[NVL_XB_SLOTS];
                             uint64_t rz_consumed[NVL_MAX_PEERS]; uint32_t rz_launched[NVL_MAX_PEERS]; nvl_xb_rz_t rz[NVL_MAX_PEERS][NVL_XB_RZ_SLOTS]; } nvl_xb_seg_t;
-typedef struct nvl_ipc_cache { unsigned n; struct { uint64_t base; cudaIpcMemHandle_t handle; void *mapped; } e[NVL_IPC_CACHE_MAX]; } nvl_ipc_cache_t;
+/* one peer allocation mapped through CUDA IPC.  refs: zero-copy plans whose tables point into it (a persistent request's cached
+ * tables until the request is finalized; any other post from its mapping to its launch).  last_use: recorded behind the latest
+ * eager launch that used it.  An entry is idle, and may be closed, once it has no refs and last_use has completed. */
+typedef struct nvl_ipc_entry { uint64_t base; size_t len; cudaIpcMemHandle_t handle; void *mapped; unsigned refs; int stale; cudaEvent_t last_use; } nvl_ipc_entry_t;
+/* per peer; holds NVL_IPC_CACHE_MAX entries, a full cache closes its idle entries and grows when none is idle */
+typedef struct nvl_ipc_cache { unsigned n, cap; nvl_ipc_entry_t **e; } nvl_ipc_cache_t;
 
 typedef struct ucc_tl_nvl_lib { ucc_tl_lib_t super; } ucc_tl_nvl_lib_t;
 
@@ -211,6 +216,7 @@ typedef struct nvl_zc {
     nvl_direct_t   d;
     uint64_t       seq;                /* board entry of the current post */
     int            published, pending; /* pending: the current post resolves through the board */
+    nvl_ipc_entry_t *pin[2 * NVL_MAX_PEERS]; unsigned npin; /* the IPC mappings the tables in d point into, referenced */
 } nvl_zc_t;
 typedef struct ucc_tl_nvl_task {
     ucc_coll_task_t     super;
@@ -261,6 +267,9 @@ char        *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const n
 void         ucc_tl_nvl_zc_init(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, unsigned flags, const void *src, size_t src_len, void *dst, size_t dst_len, const ucc_coll_args_t *reg);
 void         ucc_tl_nvl_zc_post(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int captured, const size_t *aux);
 ucc_status_t ucc_tl_nvl_zc_ready(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int persistent, const size_t *aux, size_t *aux_for_me, int *direct);
+void         ucc_tl_nvl_zc_launched(nvl_zc_t *zc, cudaStream_t s);
+void         ucc_tl_nvl_zc_release(nvl_zc_t *zc);
+void         ucc_tl_nvl_ipc_used(ucc_tl_nvl_team_t *team, ucc_rank_t p, const void *ptr, cudaStream_t s);
 
 #define NVL_CTX(_team) ucc_derived_of((_team)->super.super.context, ucc_tl_nvl_context_t)
 extern ucc_tl_iface_t ucc_tl_nvl;

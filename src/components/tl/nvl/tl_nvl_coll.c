@@ -184,6 +184,7 @@ static ucc_status_t launch_ordered(ucc_tl_nvl_task_t *t, cudaStream_t s)
     if (st != UCC_OK) return st;
     CUDA_CHECK(cudaEventRecord(t->event, s));
     team->last_event[t->lane] = t->event; team->last_stream[t->lane] = s;
+    if (t->zc.npin) ucc_tl_nvl_zc_launched(&t->zc, s);
     return UCC_OK;
 }
 
@@ -294,6 +295,7 @@ static ucc_status_t p2p_try_send(ucc_tl_nvl_task_t *t, int at_post)
         CUDA_CHECK(cudaStreamWaitEvent(team->p2p_stream[peer], t->in_event, 0));
         st = nvl_launch(t, team->p2p_stream[peer]);
         if (st != UCC_OK) return st;
+        if (t->u.p2p.mode == NVL_P2P_PUSH) ucc_tl_nvl_ipc_used(team, (ucc_rank_t)peer, t->u.p2p.remote, team->p2p_stream[peer]);
         CUDA_CHECK(cudaEventRecord(t->event, team->p2p_stream[peer]));
         CUDA_CHECK(cudaEventRecord(team->p2p_side_event[peer], team->p2p_stream[peer]));
         team->p2p_side_used[peer] = 1;
@@ -512,6 +514,7 @@ static ucc_status_t nvl_finalize(ucc_coll_task_t *ct)
     if (t->event && team->last_event[t->lane] == t->event) { /* the lane still orders its next launch after this event: keep it alive */
         cudaEvent_t spare = team->order_event[t->lane]; team->order_event[t->lane] = t->event; t->event = spare;
     }
+    ucc_tl_nvl_zc_release(&t->zc);
     ucc_spin_unlock(&team->launch_lock);
     if (t->in_event) { event_put(NVL_CTX(team), t->in_event); t->in_event = NULL; }
     if (t->event) event_put(NVL_CTX(team), t->event);
@@ -543,7 +546,7 @@ static ucc_status_t task_alloc(ucc_base_coll_args_t *b, ucc_base_team_t *b_team,
     ucc_tl_nvl_task_t *t = (ucc_tl_nvl_task_t *)ucc_mpool_get(&ctx->task_mp);
     if (!t) return UCC_ERR_NO_MEMORY;
     ucc_coll_task_init(&t->super, b, b_team);
-    t->team = team; t->path = path; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->zc.flags = 0;
+    t->team = team; t->path = path; t->event = NULL; t->captured = 0; t->lane = 0; t->in_event = NULL; t->state = NVL_TASK_LAUNCHED; t->zc.flags = 0; t->zc.npin = 0;
     t->nthreads = (int)ctx->cfg.nthreads;
     t->super.post = nvl_post; t->super.progress = nvl_progress; t->super.finalize = nvl_finalize; t->super.triggered_post = nvl_triggered_post;
     t->event = event_get(ctx);

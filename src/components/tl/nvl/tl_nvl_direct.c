@@ -49,13 +49,33 @@ ucc_status_t ucc_tl_nvl_xb_attach(ucc_tl_nvl_team_t *team)
 void ucc_tl_nvl_xb_unlink(ucc_tl_nvl_team_t *team)
 { if (team->xb_named) { ucc_shm_unlink(team->xb_name); team->xb_named = 0; } }
 
+static void entry_close(nvl_ipc_entry_t *x)
+{
+    if (cudaIpcCloseMemHandle(x->mapped) != cudaSuccess) (void)cudaGetLastError();
+    if (x->last_use) cudaEventDestroy(x->last_use);
+    free(x);
+}
+
+/* no table refers to the mapping and the last launch that used it has completed (a query: never a device synchronize, which
+ * would also invalidate a global-mode stream capture running on another thread) */
+static int entry_idle(const nvl_ipc_entry_t *x)
+{
+    cudaError_t e;
+    if (x->refs) return 0;
+    if (!x->last_use) return 1;
+    e = cudaEventQuery(x->last_use);
+    if (e == cudaSuccess) return 1;
+    (void)cudaGetLastError();
+    return 0;
+}
+
 void ucc_tl_nvl_xb_release(ucc_tl_nvl_team_t *team)
 {
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
     for (ucc_rank_t p = 0; p < N && p < NVL_MAX_PEERS; p++) {
         nvl_ipc_cache_t *c = &team->ipc_cache[p];
-        for (unsigned i = 0; i < c->n; i++) if (c->e[i].mapped) { if (cudaIpcCloseMemHandle(c->e[i].mapped) != cudaSuccess) (void)cudaGetLastError(); }
-        c->n = 0;
+        for (unsigned i = 0; i < c->n; i++) entry_close(c->e[i]);
+        free(c->e); c->e = NULL; c->n = c->cap = 0;
         if (p != me && team->xb[p]) ucc_shm_detach(team->xb[p], sizeof(nvl_xb_seg_t));
         team->xb[p] = NULL;
     }
@@ -93,35 +113,95 @@ static int xb_publish(ucc_tl_nvl_team_t *team, const nvl_zc_t *zc, int usable, c
     return 1;
 }
 
-static char *import_buf(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b)
+/* my address of the peer buffer `b`; an IPC mapping comes back referenced in *ent (NULL: nothing to release).  A full cache
+ * never closes a referenced or busy mapping: it grows instead.  Mapping happens after the members' symmetric decision to go
+ * zero-copy, so running out of room here cannot fall back to staging. */
+static char *import_buf(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b, nvl_ipc_entry_t **ent)
 {
     nvl_ipc_cache_t *c = &team->ipc_cache[p];
+    nvl_ipc_entry_t *x;
     void *mapped = NULL;
     unsigned i;
+    *ent = NULL;
     if (b->kind == NVL_XB_RAW) return (char *)(uintptr_t)b->base;
     if (b->kind != NVL_XB_IPC) return NULL;
     for (i = 0; i < c->n; i++) {
-        if (c->e[i].base != b->base) continue;
-        if (!memcmp(&c->e[i].handle, &b->handle, sizeof(b->handle))) return (char *)c->e[i].mapped + b->off;
-        /* same address, different allocation: the peer freed and re-allocated */
-        if (cudaIpcCloseMemHandle(c->e[i].mapped) != cudaSuccess) (void)cudaGetLastError();
-        c->e[i] = c->e[--c->n];
+        x = c->e[i];
+        if (x->stale || x->base != b->base) continue;
+        if (!memcmp(&x->handle, &b->handle, sizeof(b->handle))) { x->refs++; *ent = x; return (char *)x->mapped + b->off; }
+        /* same address, different allocation: the peer freed and re-allocated; a mapping still in use is closed once idle */
+        if (entry_idle(x)) { entry_close(x); c->e[i] = c->e[--c->n]; }
+        else x->stale = 1;
         break;
     }
-    if (c->n == NVL_IPC_CACHE_MAX) { /* rare: drop everything that is certainly idle */
-        cudaDeviceSynchronize();
-        for (i = 0; i < c->n; i++) if (cudaIpcCloseMemHandle(c->e[i].mapped) != cudaSuccess) (void)cudaGetLastError();
-        c->n = 0;
+    if (c->n == c->cap) {
+        for (i = 0; i < c->n;) {
+            if (entry_idle(c->e[i])) { entry_close(c->e[i]); c->e[i] = c->e[--c->n]; }
+            else i++;
+        }
     }
+    if (c->n == c->cap) {
+        unsigned cap = c->cap ? 2 * c->cap : NVL_IPC_CACHE_MAX;
+        nvl_ipc_entry_t **e = (nvl_ipc_entry_t **)realloc(c->e, cap * sizeof(*e));
+        if (!e) return NULL;
+        if (c->cap) tl_debug(NVL_LIB(team), "IPC cache of rank %u: %u mappings in use, growing to %u", p, c->n, cap);
+        c->e = e; c->cap = cap;
+    }
+    x = (nvl_ipc_entry_t *)calloc(1, sizeof(*x));
+    if (!x) return NULL;
     if (cudaIpcOpenMemHandle(&mapped, b->handle, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
         tl_debug(NVL_LIB(team), "cudaIpcOpenMemHandle of a buffer of rank %u failed: %s", p, cudaGetErrorString(cudaGetLastError()));
+        free(x);
         return NULL;
     }
-    c->e[c->n].base = b->base; c->e[c->n].handle = b->handle; c->e[c->n].mapped = mapped; c->n++;
+    x->base = b->base; x->len = b->alloc_len; x->handle = b->handle; x->mapped = mapped; x->refs = 1;
+    c->e[c->n++] = x;
+    *ent = x;
     return (char *)mapped + b->off;
 }
 
-char *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b) { return import_buf(team, p, b); }
+/* a mapping for one launch that follows right away: the caller reports that launch with ucc_tl_nvl_ipc_used() before it maps
+ * anything else */
+char *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b)
+{
+    nvl_ipc_entry_t *x;
+    char *r = import_buf(team, p, b, &x);
+    if (x) x->refs--;
+    return r;
+}
+
+static void entry_used(nvl_ipc_entry_t *x, cudaStream_t s)
+{
+    if (!x->last_use && cudaEventCreateWithFlags(&x->last_use, cudaEventDisableTiming) != cudaSuccess) { (void)cudaGetLastError(); x->last_use = NULL; x->refs++; return; } /* untracked: never idle */
+    if (cudaEventRecord(x->last_use, s) != cudaSuccess) { (void)cudaGetLastError(); x->refs++; }
+}
+
+/* the kernel just launched on s reads or writes `ptr`, which ucc_tl_nvl_xb_import() mapped from rank p */
+void ucc_tl_nvl_ipc_used(ucc_tl_nvl_team_t *team, ucc_rank_t p, const void *ptr, cudaStream_t s)
+{
+    nvl_ipc_cache_t *c = &team->ipc_cache[p];
+    for (unsigned i = 0; i < c->n; i++) {
+        nvl_ipc_entry_t *x = c->e[i];
+        if ((const char *)ptr >= (const char *)x->mapped && (const char *)ptr < (const char *)x->mapped + x->len) { entry_used(x, s); return; }
+    }
+}
+
+static void zc_unpin(nvl_zc_t *zc)
+{
+    for (unsigned i = 0; i < zc->npin; i++) zc->pin[i]->refs--;
+    zc->npin = 0;
+}
+
+/* the direct form of the current post was launched on s (not captured: a captured post only runs tables that a persistent
+ * request cached, and they stay referenced until it is finalized).  Tables resolved for this post only are released. */
+void ucc_tl_nvl_zc_launched(nvl_zc_t *zc, cudaStream_t s)
+{
+    for (unsigned i = 0; i < zc->npin; i++) entry_used(zc->pin[i], s);
+    if (zc->cache != NVL_ZC_DIRECT) zc_unpin(zc);
+}
+
+/* at finalize: the request's tables are no longer used by any future launch */
+void ucc_tl_nvl_zc_release(nvl_zc_t *zc) { zc_unpin(zc); }
 
 /* Registered buffers: when the collective carries GLOBAL memory handles (one imported ucc_mem_map handle per member) for every
  * side the zero-copy kernel touches, the pointer tables are built at init from the registrations - the per-post exchange is
@@ -160,7 +240,7 @@ static int memh_tables(ucc_tl_nvl_team_t *team, const ucc_coll_args_t *a, nvl_zc
  * `reg`: the arguments whose registrations may give the tables (NULL: never) */
 void ucc_tl_nvl_zc_init(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, unsigned flags, const void *src, size_t src_len, void *dst, size_t dst_len, const ucc_coll_args_t *reg)
 {
-    zc->flags = flags; zc->src = src; zc->src_len = src_len; zc->dst = dst; zc->dst_len = dst_len;
+    zc->flags = flags; zc->src = src; zc->src_len = src_len; zc->dst = dst; zc->dst_len = dst_len; zc->npin = 0;
     zc->cache = reg && memh_tables(team, reg, zc) ? NVL_ZC_DIRECT : NVL_ZC_RESOLVE;
     if (zc->cache == NVL_ZC_RESOLVE && !team->zcopy) zc->flags = 0; /* no board and nothing cached: always staged */
 }
@@ -202,12 +282,15 @@ ucc_status_t ucc_tl_nvl_zc_ready(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int pers
     /* up to here every member took the same decision (it only depends on what all of them published).  Mapping a peer's
      * allocation can still fail on THIS rank only; the peers will launch the in-place kernel, so falling back to the staged
      * one here would mix two protocols and corrupt data silently: fail the collective. */
+    zc_unpin(zc);
     for (ucc_rank_t p = 0; p < N && ok > 0; p++) {
         const nvl_xb_entry_t *e = &team->xb[p]->e[zc->seq % NVL_XB_SLOTS];
+        nvl_ipc_entry_t *x;
         if (p == me) { d->src[p] = (const char *)zc->src; d->dst[p] = (char *)zc->dst; continue; }
-        if (need_src && e->src.kind != NVL_XB_EMPTY) { d->src[p] = import_buf(team, p, &e->src); if (!d->src[p]) ok = -1; }
-        if (need_dst && e->dst.kind != NVL_XB_EMPTY) { d->dst[p] = import_buf(team, p, &e->dst); if (!d->dst[p]) ok = -1; }
+        if (need_src && e->src.kind != NVL_XB_EMPTY) { d->src[p] = import_buf(team, p, &e->src, &x); if (x) zc->pin[zc->npin++] = x; if (!d->src[p]) ok = -1; }
+        if (need_dst && e->dst.kind != NVL_XB_EMPTY) { d->dst[p] = import_buf(team, p, &e->dst, &x); if (x) zc->pin[zc->npin++] = x; if (!d->dst[p]) ok = -1; }
     }
+    if (ok < 0) zc_unpin(zc);
     if (team->xb_mine->consumed < zc->seq + 1) ucc_store_release(&team->xb_mine->consumed, zc->seq + 1);
     tl_debug(NVL_LIB(team), "exchange %lu: %s (src %d dst %d)", (unsigned long)zc->seq, ok > 0 ? "zero-copy" : (ok ? "MAPPING FAILED" : "staged"),
              !!need_src, !!need_dst);
@@ -219,7 +302,7 @@ ucc_status_t ucc_tl_nvl_zc_ready(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, int pers
     zc->pending = 0;
     /* persistent request: the buffers are fixed for the lifetime of the request, so every later post of it (same decision on
      * every member - they all re-post the same request) launches straight away with these tables: no handle export, no board
-     * round trip, no deferred launch */
+     * round trip, no deferred launch.  Its mappings stay referenced until the request is finalized (ucc_tl_nvl_zc_release). */
     if (persistent) zc->cache = ok ? NVL_ZC_DIRECT : NVL_ZC_STAGED;
     *direct = ok;
     return UCC_OK;

@@ -323,7 +323,7 @@ static ucc_status_t team_finish(ucc_tl_nvl_team_t *team)
     team->dev.timeout_ns = (uint64_t)(ctx->cfg.timeout * 1e9);
     { void *dptr = NULL; CUDA_CHECK(cudaHostGetDevicePointer(&dptr, team->host_err, 0)); team->dev.host_err = (uint32_t *)dptr; }
     team->state = NVL_TEAM_READY;
-    if (!team->self && ctx->cfg.user_size) registry_add(team);
+    registry_add(team);
     tl_debug(NVL_LIB(team), "team %p ready: size %u, heap %s %zu MB, nvls %d", (void *)team, N,
              team->heap_kind == NVL_HEAP_LOCAL ? "local" : team->heap_kind == NVL_HEAP_VMM ? "vmm" : "ipc", team->heap_size >> 20, team->nvls);
     return UCC_OK;
@@ -418,8 +418,9 @@ fail:
 /* ------------------------------------------------------------------ */
 /* symmetric user region                                               */
 /* ------------------------------------------------------------------ */
-/* ready teams, so that an application holding only the ucc_team_h can ask for the user region of the tl/nvl team that spans it */
-#define NVL_REG_MAX 64
+/* ready teams, so that an application holding only the ucc_team_h can ask for the user region of the tl/nvl team that spans it,
+ * or for its device-error latch */
+#define NVL_REG_MAX 1024
 static ucc_tl_nvl_team_t *g_teams[NVL_REG_MAX];
 static ucc_spinlock_t     g_teams_lock;
 static void registry_add(ucc_tl_nvl_team_t *team)
@@ -438,13 +439,31 @@ UCC_EXPORT ucc_status_t ucc_tl_nvl_symm_region(ucc_team_h core_team, void **base
     for (int i = 0; i < NVL_REG_MAX; i++) {
         ucc_tl_nvl_team_t *t = g_teams[i];
         if (!t || t->self || (ucc_team_h)t->super.super.params.team != core_team || UCC_TL_TEAM_SIZE(t) != ucc_team_size_(core_team)) continue;
-        if (!NVL_CTX(t)->cfg.user_size) { st = UCC_ERR_NOT_SUPPORTED; continue; }
+        if (!NVL_CTX(t)->cfg.user_size) continue;
         *base = t->heap + t->lane_stride * t->nlanes; *size = NVL_CTX(t)->cfg.user_size;
         if (nvls) *nvls = t->nvls;
         st = UCC_OK; break;
     }
     ucc_spin_unlock(&g_teams_lock);
     return st;
+}
+
+/* Reads and clears the device-error latch of every tl/nvl team of `core_team`: 1 when a kernel of one of them gave up a
+ * device-side wait (TL_NVL_TIMEOUT) since the last call, 0 otherwise, -1 when the core team has no tl/nvl team.  An eager
+ * collective reports such a timeout through its request; a collective replayed from a CUDA graph has no request, so an
+ * application that replays graphs asks here after synchronizing the replay stream. */
+UCC_EXPORT int ucc_tl_nvl_take_device_error(ucc_team_h core_team)
+{
+    int r = -1;
+    ucc_spin_lock(&g_teams_lock);
+    for (int i = 0; i < NVL_REG_MAX; i++) {
+        ucc_tl_nvl_team_t *t = g_teams[i];
+        if (!t || (ucc_team_h)t->super.super.params.team != core_team) continue;
+        if (r < 0) r = 0;
+        if (t->host_err && __atomic_exchange_n(t->host_err, 0, __ATOMIC_ACQ_REL)) r = 1;
+    }
+    ucc_spin_unlock(&g_teams_lock);
+    return r;
 }
 
 ucc_status_t ucc_tl_nvl_team_destroy(ucc_base_team_t *b)

@@ -2,12 +2,14 @@
 # The full tl/nvl stack in the host emulation (tests/test_nvl_hostemu.py, test_nvl_complex.py, test_nvl_swap.py) under ThreadSanitizer
 # and AddressSanitizer: the plugin's host code (team creation, launch queue, exchange board, ...) cannot be sanitised on a GPU box
 # without the CUDA runtime getting in the way; against the emulated runtime it can.
-# A run is a scenario of tests/hostemu_worker.py, or worker:scenario for tests/hostemu_<worker>_worker.py.
+# A run is a scenario of tests/hostemu_worker.py, or worker:scenario for tests/hostemu_<worker>_worker.py (graph:graphs runs on the
+# graph build of the plugin, tests/emu/build_hostemu_graph.sh).
 cd "$(dirname "$0")/.."
 export EMU_CC=/usr/bin/gcc EMU_CXX=/usr/bin/g++
 rc=0
 for san in thread address; do
   EMU_EXTRA="-fsanitize=$san -g" tests/emu/build_hostemu.sh > /dev/null 2>&1 || { echo "build failed ($san)"; exit 1; }
+  EMU_EXTRA="-fsanitize=$san -g" tests/emu/build_hostemu_graph.sh > /dev/null 2>&1 || { echo "graph build failed ($san)"; exit 1; }
   rm -f /tmp/ucc_b200_he_$san.*
   lib=$(/usr/bin/gcc -print-file-name=$([ $san = thread ] && echo libtsan.so || echo libasan.so))
   for s in ${HOSTEMU_SCENARIOS:-allreduce colls_staged colls_zcopy colls_push colls_ce misc triggered p2p memh lanes complex: \
@@ -22,5 +24,5 @@ for san in thread address; do
   n=$(ls /tmp/ucc_b200_he_$san.* 2>/dev/null | wc -l)
   echo "$san: sanitizer report files: $n"; [ "$n" = 0 ] || rc=1
 done
-tests/emu/build_hostemu.sh > /dev/null 2>&1   # back to the plain build
+tests/emu/build_hostemu.sh > /dev/null 2>&1; tests/emu/build_hostemu_graph.sh > /dev/null 2>&1   # back to the plain builds
 exit $rc

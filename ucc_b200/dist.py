@@ -4,6 +4,7 @@ torch.distributed (gloo) only provides the out-of-band allgather used for wire-u
 MPI plays for the reference's ucc_perftest (tools/perf/ucc_pt_bootstrap_mpi.cc).  All collectives
 then run through libucc: tl/nvl kernels over NVLink for CUDA tensors, tl/shm for host tensors.
 """
+import contextlib
 import ctypes as C
 import itertools
 import os
@@ -108,9 +109,33 @@ class MemHandles:
         self._imported, self._blobs = [], []
 
 
+_cu_capture_mode = None
+
+
+@contextlib.contextmanager
+def _relaxed_capture():
+    """While the current stream captures a CUDA graph, progress polls the completion events of eager collectives
+    (cudaEventQuery), which a capture in the default global mode forbids on every thread: switch this thread to relaxed mode
+    for the duration, as PyTorch's own NCCL watchdog does."""
+    global _cu_capture_mode
+    if not (torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()):
+        yield
+        return
+    if _cu_capture_mode is None:
+        _cu_capture_mode = C.CDLL("libcuda.so.1").cuThreadExchangeStreamCaptureMode
+        _cu_capture_mode.argtypes = [C.POINTER(C.c_int)]
+    mode = C.c_int(2)   # CU_STREAM_CAPTURE_MODE_RELAXED
+    _cu_capture_mode(C.byref(mode))
+    try:
+        yield
+    finally:
+        _cu_capture_mode(C.byref(mode))
+
+
 class Request:
     def __init__(self, comm, req, keep):
         self.comm, self.req, self._keep = comm, req, keep
+        self._graphed = False      # owned by the communicator's graphed() cache: finalize() leaves it alone
 
     def post(self):
         U.check(U.ucc_collective_post(self.req), "collective_post")
@@ -121,13 +146,19 @@ class Request:
 
         With `wait_posted` the call returns once UCC_EVENT_COLLECTIVE_POST was delivered, i.e. the kernel really is
         in the stream (a zero-copy collective first learns the peers' buffer mappings, which takes a few host
-        microseconds); work enqueued on the stream afterwards is ordered behind the collective."""
+        microseconds); work enqueued on the stream afterwards is ordered behind the collective.
+
+        Inside `torch.cuda.graph` the kernel is captured, not run: the post returns as soon as it is in the graph and the
+        request completes at once.  Every replay of the graph runs the collective again."""
+        if self._graphed and self.req.contents.status == U.UCC_INPROGRESS:
+            self.wait()            # a persistent request is posted again only once its previous post completed
         ev = U.ucc_ev_t()
         ev.ev_type = U.UCC_EVENT_COMPUTE_COMPLETE
         ev.req = C.cast(self.req, C.c_void_p)
         self._ee = self.comm.ee_for(stream)
         self._seen_posted = False
         U.check(U.ucc_collective_triggered_post(self._ee, C.byref(ev)), "triggered_post")
+        self.comm._unposted.add(self)
         if wait_posted:
             self.wait_posted()
         return self
@@ -137,29 +168,38 @@ class Request:
         if getattr(self, "_seen_posted", False):
             return
         key = C.cast(self.req, C.c_void_p).value
-        while key not in self.comm._posted:
-            st = self.req.contents.status
-            if st < 0:
-                raise U.UccError(st, "collective")
-            if not self.comm.collect_events(self._ee):
-                U.ucc_context_progress(self.comm.ctx)
+        with _relaxed_capture():
+            while key not in self.comm._posted:
+                st = self.req.contents.status
+                if st < 0:
+                    raise U.UccError(st, "collective")
+                if not self.comm.collect_events(self._ee):
+                    U.ucc_context_progress(self.comm.ctx)
         self.comm._posted.discard(key)
+        self.comm._unposted.discard(self)
         self._seen_posted = True
 
     def test(self):
         return self.req.contents.status
 
     def wait(self):
-        while True:
-            st = self.req.contents.status
-            if st == U.UCC_OK:
-                return
-            if st < 0:
-                raise U.UccError(st, "collective")
-            U.ucc_context_progress(self.comm.ctx)
+        with _relaxed_capture():
+            while True:
+                st = self.req.contents.status
+                if st == U.UCC_OK:
+                    return
+                if st < 0:
+                    raise U.UccError(st, "collective")
+                U.ucc_context_progress(self.comm.ctx)
 
     def finalize(self):
+        if self._graphed:
+            return
+        self._release()
+
+    def _release(self):
         self.comm.drain_events()
+        self.comm._unposted.discard(self)
         U.check(U.ucc_collective_finalize(self.req), "collective_finalize")
         self.req = None
 
@@ -229,6 +269,51 @@ class Communicator:
             U.ucc_context_progress(self.ctx)
         self._ees = {}
         self._posted = set()
+        self._unposted = set()     # stream-ordered posts whose kernel may not be in its stream yet
+        self._graphing = 0
+        self._graph_reqs = {}
+
+    # ------------------------------------------------------------------ CUDA graphs
+    @contextlib.contextmanager
+    def graphed(self):
+        """Collectives for a CUDA graph: use it around the warm-up iterations AND the capture.
+
+            with comm.graphed():
+                for _ in range(3):                      # warm-up, eager (on a side stream, as torch.cuda.graph wants)
+                    step()
+                with torch.cuda.graph(g):
+                    step()
+            g.replay()                                 # any number of times, on every member, in the same order
+
+        Inside, every collective of this communicator (and of `ops` / the torch backend on top of it) is a persistent request,
+        cached by its arguments: collective, buffer addresses, counts, datatype, operator, root.  The warm-up posts of a
+        request resolve the zero-copy tables of the members' buffers, and the captured post reuses them, so the graph runs
+        large collectives in place instead of staging them through the team heap.  A collective first posted under capture
+        runs staged.  The requests stay alive, and the graph valid, until release_graphed() or destroy().  On entry, the
+        collectives already posted are waited into their streams: a capture must not begin while a launch is still queued."""
+        for r in list(self._unposted):
+            r.wait_posted()
+        self._graphing += 1
+        try:
+            yield self
+        finally:
+            self._graphing -= 1
+
+    def release_graphed(self):
+        """finalize the requests cached by graphed(); graphs captured from them must not be replayed any more"""
+        reqs, self._graph_reqs = list(self._graph_reqs.values()), {}
+        for r in reqs:
+            r.wait()
+            r._release()
+
+    def take_device_error(self):
+        """True when a tl/nvl kernel of this team gave up a device-side wait (UCC_TL_NVL_TIMEOUT) since the last call.  A
+        replayed collective has no request to carry the error: call this after synchronizing the replay stream."""
+        fn = getattr(self, "_dev_err_fn", None)
+        if fn is None:
+            fn = self._dev_err_fn = C.CDLL(os.path.join(os.path.dirname(U.LIB_PATH), "ucc", "libucc_tl_nvl.so")).ucc_tl_nvl_take_device_error
+            fn.restype, fn.argtypes = C.c_int, [U.handle]
+        return fn(self.team) == 1
 
     # ------------------------------------------------------------------ symmetric user memory (tl/nvl)
     def symm_region(self):
@@ -323,6 +408,23 @@ class Communicator:
         U.check(U.ucc_collective_init(C.byref(args), C.byref(r), self.team), "collective_init")
         return Request(self, r, (args, hold))   # `hold` keeps the tensors alive until the request is finalized
 
+    def _init_cached(self, key, make_args, hold):
+        """init() outside graphed(); inside, the persistent request cached under `key` (created on first use)"""
+        if not self._graphing:
+            return self.init(make_args(False), hold)
+        req = self._graph_reqs.get(key)
+        if req is None:
+            req = self.init(make_args(True), hold)
+            req._graphed = True
+            self._graph_reqs[key] = req
+        return req
+
+    @staticmethod
+    def _graph_key(coll, src, dst, kw):
+        def desc(t):
+            return None if t is None else (t.data_ptr(), t.numel(), t.dtype, str(t.device))
+        return (coll, desc(src), desc(dst)) + tuple(sorted((k, tuple(v) if isinstance(v, (list, tuple)) else v) for k, v in kw.items()))
+
     def _args(self, coll, src=None, dst=None, op="sum", root=0, inplace=False, persistent=False, **kw):
         from .harness import coll_args
         ref = dst if dst is not None else src
@@ -361,20 +463,25 @@ class Communicator:
 
     def allreduce_init(self, src, dst, op="sum", persistent=False):
         inplace = src is None or src.data_ptr() == dst.data_ptr()
-        return self.init(self._args("allreduce", None if inplace else src, dst, op=op, inplace=inplace, persistent=persistent), (src, dst))
+        s = None if inplace else src
+        return self._init_cached(self._graph_key("allreduce", s, dst, {"op": op}),
+                                 lambda p: self._args("allreduce", s, dst, op=op, inplace=inplace, persistent=persistent or p), (src, dst))
 
     def coll_init(self, coll, src=None, dst=None, src_memh=None, dst_memh=None, **kw):
         """`src_memh` / `dst_memh`: MemHandles from register() - the buffers are parts of registered segments"""
-        a = self._args(coll, src, dst, **kw)
-        if src_memh is not None:
-            a.mask |= U.UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | U.UCC_COLL_ARGS_FIELD_FLAGS
-            a.flags |= U.UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL
-            a.src_memh.global_memh = C.cast(src_memh.array, C.POINTER(C.c_void_p))
-        if dst_memh is not None:
-            a.mask |= U.UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH | U.UCC_COLL_ARGS_FIELD_FLAGS
-            a.flags |= U.UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL
-            a.dst_memh.global_memh = C.cast(dst_memh.array, C.POINTER(C.c_void_p))
-        return self.init(a, (src, dst, src_memh, dst_memh))
+        def make(persistent):
+            a = self._args(coll, src, dst, **dict(kw, persistent=kw.get("persistent", False) or persistent))
+            if src_memh is not None:
+                a.mask |= U.UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | U.UCC_COLL_ARGS_FIELD_FLAGS
+                a.flags |= U.UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL
+                a.src_memh.global_memh = C.cast(src_memh.array, C.POINTER(C.c_void_p))
+            if dst_memh is not None:
+                a.mask |= U.UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH | U.UCC_COLL_ARGS_FIELD_FLAGS
+                a.flags |= U.UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL
+                a.dst_memh.global_memh = C.cast(dst_memh.array, C.POINTER(C.c_void_p))
+            return a
+        key = self._graph_key(coll, src, dst, dict(kw, src_memh=id(src_memh), dst_memh=id(dst_memh)))
+        return self._init_cached(key, make, (src, dst, src_memh, dst_memh))
 
     def run(self, req, stream=None):
         """Convenience: post, wait (host), finalize."""
@@ -385,6 +492,7 @@ class Communicator:
         self.run(self.coll_init("barrier"))
 
     def destroy(self):
+        self.release_graphed()
         for ee in self._ees.values():
             U.ucc_ee_destroy(ee)
         self._ees = {}

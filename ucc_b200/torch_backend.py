@@ -8,7 +8,10 @@
 
 The process group is a Python subclass of `torch.distributed.ProcessGroup`; wire-up uses the rendezvous store as the
 UCC out-of-band allgather.  CUDA collectives are posted stream-ordered on the caller's current stream, so `Work.wait()`
-only has to make sure the kernel is in the stream (it does not block the host on the GPU)."""
+only has to make sure the kernel is in the stream (it does not block the host on the GPU).
+
+Every collective works inside `torch.cuda.graph`.  Wrap the warm-up iterations and the capture in `pg.graphed()` (see
+Communicator.graphed) so that the captured collectives reuse the zero-copy tables their warm-up posts resolved."""
 from __future__ import annotations
 
 import torch
@@ -79,6 +82,13 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     def getBackendName(self):
         return "ucc_b200"
 
+    def graphed(self):
+        """context manager for the warm-up and the capture of a CUDA graph: Communicator.graphed() of this group"""
+        return self._comm.graphed()
+
+    def release_graphed(self):
+        self._comm.release_graphed()
+
     # ---- helpers
     def _run(self, reqs, tensors, result, wait_posted=True):
         cuda = bool(tensors) and tensors[0].is_cuda
@@ -94,6 +104,8 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     def _reap(self):
         keep = []
         for r in self._pending:
+            if r._graphed:          # owned by the graphed() cache, which finalizes it
+                continue
             if r.test() == 0:
                 r.finalize()
             else:
@@ -207,7 +219,8 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     def shutdown(self):
         for r in self._pending:
-            r.wait(); r.finalize()
+            if not r._graphed:
+                r.wait(); r.finalize()
         self._pending = []
         self._comm.destroy()
 
