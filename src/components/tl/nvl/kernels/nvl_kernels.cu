@@ -248,8 +248,8 @@ extern "C" cudaError_t nvl_launch_ctrl_init(void *heap_base, cudaStream_t s)
     return cudaGetLastError();
 }
 #elif defined(NVL_EMU_LAUNCHERS)
-/* the host-emulated plugin (tests/emu/nvl_emu_launch.cpp) defines a table of the datatypes it builds and a run on its emulated
- * stream */
+/* the host-emulated plugin (tests/emu/nvl_emu_launch.cpp, one for every CPU test) defines a table of the datatypes it builds and a
+ * run on its emulated stream, which refuses a kernel whose tables reach into a closed IPC mapping */
 extern const nvl_dt_row *const nvl_rows[NVL_DT_LAST];
 static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nblocks, int nthreads, cudaStream_t s);
 #endif /* NVL_HOST_EMU */

@@ -1,5 +1,5 @@
 """Worker of tests/test_nvl_graph.py: tl/nvl collectives captured into CUDA graphs and replayed, on the host-emulated plugin built by
-tests/emu/build_hostemu_graph.sh, whose CUDA runtime emulates stream capture: a capturing stream records kernels, copies and
+tests/emu/build_hostemu.sh, whose CUDA runtime emulates stream capture: a capturing stream records kernels, copies and
 memsets, and a graph launch replays them in order.  Every rank captures its sequence on its own stream, one rank after the other (a
 captured post never waits for the peers), then all ranks replay together; every result is checked exactly against numpy."""
 import ctypes as C
@@ -10,50 +10,10 @@ import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-os.environ["UCC_MODULE_DIR"] = os.path.join(ROOT, "build-emu", "lib_graph", "ucc")
-faulthandler.dump_traceback_later(900, exit=True)
-rt = C.CDLL(os.path.join(ROOT, "build-emu", "lib_graph", "libcudart_emu.so"), mode=C.RTLD_GLOBAL)
-sys.path.insert(0, ROOT)
-from ucc_b200 import capi as U  # noqa: E402
-from ucc_b200.harness import UccJob, coll_args  # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from hostemu_worker import BASE, NOZC, ZC, Dev, U, UccJob, ca, last_launch, rnd, rt  # noqa: E402  (loads the emulated runtime)
 
-CUDA = U.UCC_MEMORY_TYPE_CUDA
-BASE = {"UCC_TL_NVL_MAX_BLOCKS": "2", "UCC_TL_NVL_NTHREADS": "64", "UCC_TL_NVL_TIMEOUT": "30s", "UCC_TL_NVL_SYMMETRIC_SIZE": "1Mb", "UCC_TLS": "nvl,shm,self",
-        "UCC_COLL_TRACE": "info"}
-ZC = {"UCC_TL_NVL_ZCOPY": "y", "UCC_TL_NVL_ZCOPY_THRESH": "0"}
-NOZC = {"UCC_TL_NVL_ZCOPY": "n"}
-
-
-class Dev:
-    """numpy view of a buffer allocated with the emulated cudaMalloc"""
-
-    def __init__(self, n, dtype=np.float32, fill=None):
-        p = C.c_void_p()
-        nbytes = max(n, 1) * np.dtype(dtype).itemsize
-        assert rt.cudaMalloc(C.byref(p), C.c_size_t(nbytes)) == 0
-        self.ptr = p.value
-        self.a = np.frombuffer((C.c_char * nbytes).from_address(p.value), dtype=dtype)[:n]
-        if fill is not None:
-            self.a[:] = fill
-
-
-def ca(coll, src, dst, dt="float32", **kw):
-    kw.setdefault("count_src", src.a.size if src is not None else 0)
-    kw.setdefault("count_dst", dst.a.size if dst is not None else 0)
-    return coll_args(coll, dt=dt, mem_type=CUDA, src_ptr=src.ptr if src is not None else None, dst_ptr=dst.ptr if dst is not None else None, **kw)
-
-
-def last_launch():
-    """the launch note of the plugin's most recent kernel launch: names the kernel that served it"""
-    info = C.CDLL(os.path.join(os.environ["UCC_MODULE_DIR"], "libucc_tl_nvl.so")).ucc_tl_nvl_last_launch_info
-    info.restype = C.c_char_p
-    return info().decode()
-
-
-def rnd(n, seed, dtype=np.float32):
-    return np.random.default_rng(seed).integers(0, 9, n).astype(dtype)
-
+faulthandler.dump_traceback_later(900, exit=True)   # the whole graph scenario is one run: more time than hostemu_worker's 240 s
 
 for _f, _a in (("cudaStreamCreate", [C.POINTER(C.c_void_p)]), ("cudaStreamBeginCapture", [C.c_void_p, C.c_int]),
                ("cudaStreamEndCapture", [C.c_void_p, C.POINTER(C.c_void_p)]), ("cudaGraphInstantiate", [C.POINTER(C.c_void_p), C.c_void_p, C.c_ulonglong]),

@@ -1,6 +1,7 @@
 """Worker of tests/test_nvl_numerics.py: the numerical contract of tests/nvl_numerics.py on the tl/nvl plugin built against the
 emulated CUDA runtime (tests/emu/build_hostemu.sh), N ranks in this process.  `hostemu_numerics_worker.py <path>` runs allreduce,
-reduce_scatter(v) and reduce on one path (nvl_numerics.PATHS) for teams of 2..5, the eight datatypes the emulated plugin builds."""
+reduce_scatter(v) and reduce on one path (nvl_numerics.PATHS) for teams of 2..5, the eight datatypes the emulated plugin builds
+besides INT128 / UINT128 (those: hostemu_int128_worker.py)."""
 import os
 import sys
 

@@ -11,14 +11,19 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+_built = []
 
 
 @pytest.fixture(scope="module")
 def emu_build():
+    """the host-emulated runtime and plugin; every module that imports this fixture shares one build per session"""
     if not os.path.exists("/usr/local/cuda/include/cuda_fp16.h"):
         pytest.skip("CUDA headers not installed")
+    if _built:
+        return
     out = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu.sh")], capture_output=True, text=True, timeout=900)
     assert "HOSTEMU_BUILD_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-3000:]
+    _built.append(True)
 
 
 @pytest.mark.parametrize("scenario", ["allreduce", "colls_staged", "colls_zcopy", "colls_push", "colls_ce", "colls_ring", "misc", "triggered", "cross_team", "timeout", "p2p", "p2p_fuzz", "coll_fuzz", "memh", "lanes", "defaults", "hier"])

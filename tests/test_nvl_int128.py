@@ -35,15 +35,8 @@ def test_int128_datatype_table():
     assert lib.nvl_dt_size(len(dts)) == 0 and not lib.nvl_dt_supports_op(len(dts), 0)
 
 
-@pytest.fixture(scope="module")
-def emu_int128_build(emu_build):  # noqa: F811
-    """the host-emulated plugin with INT128 / UINT128 in its datatype table, linked from the objects emu_build compiled"""
-    out = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu_int128.sh")], capture_output=True, text=True, timeout=900)
-    assert "HOSTEMU_INT128_BUILD_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-3000:]
-
-
 @pytest.mark.parametrize("path", ["oneshot", "twoshot", "zcopy", "ring", "rhd"])
-def test_int128_reductions_host_emulation(emu_int128_build, path):
+def test_int128_reductions_host_emulation(emu_build, path):  # noqa: F811
     env = dict(os.environ, PYTHONPATH=ROOT)
     for k in ("UCC_TL_NVL_TUNE", "UCC_MODULE_DIR", "UCC_TLS"):
         env.pop(k, None)

@@ -2,13 +2,13 @@
 
 Teams inside one process publish raw pointers and never map anything, so the driver plays both members of a two-member team
 itself: two team objects share their exchange boards, and every buffer goes through the emulated cudaIpcGetMemHandle /
-cudaIpcOpenMemHandle of tests/emu/cudart_emu_graph.cpp.  A persistent allreduce resolves the zero-copy (direct) tables on its first post; then more distinct peer
+cudaIpcOpenMemHandle of tests/emu/cudart_emu.cpp.  A persistent allreduce resolves the zero-copy (direct) tables on its first post; then more distinct peer
 allocations than the cache holds are mapped, and the persistent request's tables are launched again.  The mappings those tables
 point into must still be open: the emulated launcher refuses a kernel whose tables reach into a closed mapping."""
 import os
 import subprocess
 
-import pytest
+from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -99,19 +99,11 @@ int main(void)
 '''
 
 
-@pytest.fixture(scope="module")
-def emu_build():
-    if not os.path.exists("/usr/local/cuda/include/cuda_fp16.h"):
-        pytest.skip("CUDA headers not installed")
-    out = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu_graph.sh")], capture_output=True, text=True, timeout=900)
-    assert "HOSTEMU_GRAPH_BUILD_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-3000:]
-
-
-def test_persistent_tables_survive_a_full_ipc_cache(emu_build, tmp_path):
+def test_persistent_tables_survive_a_full_ipc_cache(emu_build, tmp_path):  # noqa: F811
     src = tmp_path / "ipc_cache.c"
     src.write_text(SRC)
     exe = tmp_path / "ipc_cache"
-    emu = os.path.join(ROOT, "build-emu", "lib_graph")
+    emu = os.path.join(ROOT, "build-emu", "lib")
     core = os.path.join(ROOT, "ucc_b200", "lib")
     cc = subprocess.run(["gcc", "-O1", "-g", "-std=gnu11", "-D_GNU_SOURCE", f"-I{ROOT}/src", f"-I{ROOT}/include", "-I/usr/local/cuda/include", str(src), "-o", str(exe),
                          os.path.join(emu, "ucc", "libucc_tl_nvl.so"), f"-L{emu}", "-lcudart_emu", f"-L{core}", "-lucc",

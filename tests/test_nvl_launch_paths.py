@@ -7,21 +7,13 @@ import os
 import subprocess
 import sys
 
-import pytest
+from test_nvl_hostemu import emu_build  # noqa: F401  (module fixture: builds the host-emulated runtime and plugin)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "nvl_launch_paths.txt")
 
 
-@pytest.fixture(scope="module")
-def emu_plugin():
-    if not os.path.exists("/usr/local/cuda/include/cuda_fp16.h"):
-        pytest.skip("CUDA headers not installed")
-    out = subprocess.run(["bash", os.path.join(ROOT, "tests", "emu", "build_hostemu.sh")], capture_output=True, text=True, timeout=900)
-    assert "HOSTEMU_BUILD_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-3000:]
-
-
-def test_launch_paths_match_golden(emu_plugin):
+def test_launch_paths_match_golden(emu_build):  # noqa: F811
     env = dict(os.environ, PYTHONPATH=ROOT)
     for k in ("UCC_TL_NVL_TUNE", "UCC_MODULE_DIR", "UCC_TLS"):
         env.pop(k, None)
