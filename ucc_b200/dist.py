@@ -16,14 +16,27 @@ from . import capi as U
 
 _TORCH_DT = {torch.int8: "int8", torch.int16: "int16", torch.int32: "int32", torch.int64: "int64", torch.uint8: "uint8",
              torch.float16: "float16", torch.float32: "float32", torch.float64: "float64", torch.bfloat16: "bfloat16",
-             torch.complex64: "float32_complex", torch.complex128: "float64_complex"}
+             torch.complex64: "float32_complex", torch.complex128: "float64_complex", torch.bool: "uint8"}
 for _n, _t in (("uint16", "uint16"), ("uint32", "uint32"), ("uint64", "uint64")):
     if hasattr(torch, _n):
         _TORCH_DT[getattr(torch, _n)] = _t
 
+# a torch.bool tensor goes to the library as uint8 holding 0 / 1: sum is logical or (max), product logical and (min), as in
+# ProcessGroupNCCL; the bitwise and logical operators keep 0 / 1 as they are
+_BOOL_OP = {"sum": "max", "prod": "min"}
+
 
 def dt_of(t):
     return _TORCH_DT[t.dtype]
+
+
+def op_of(op, t):
+    """the library operator that computes `op` on the elements of `t`"""
+    if t.dtype != torch.bool:
+        return op
+    if op == "avg":
+        raise ValueError("AVG reduction is not defined for torch.bool tensors")
+    return _BOOL_OP.get(op, op)
 
 
 def mem_type_of(t):
@@ -430,7 +443,7 @@ class Communicator:
         ref = dst if dst is not None else src
         if ref is None:  # barrier / fanin / fanout
             return coll_args(coll, root=root, persistent=persistent)
-        return coll_args(coll, dt=dt_of(ref), op=op, root=root, inplace=inplace, persistent=persistent,
+        return coll_args(coll, dt=dt_of(ref), op=op_of(op, ref), root=root, inplace=inplace, persistent=persistent,
                          src_ptr=src.data_ptr() if src is not None else None, dst_ptr=dst.data_ptr() if dst is not None else None,
                          count_src=src.numel() if src is not None else 0, count_dst=dst.numel() if dst is not None else 0,
                          mem_type=mem_type_of(ref), **kw)

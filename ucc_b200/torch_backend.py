@@ -10,9 +10,19 @@ The process group is a Python subclass of `torch.distributed.ProcessGroup`; wire
 UCC out-of-band allgather.  CUDA collectives are posted stream-ordered on the caller's current stream, so `Work.wait()`
 only has to make sure the kernel is in the stream (it does not block the host on the GPU).
 
+c10d operations served: allreduce (+ _coalesced), broadcast, reduce, allgather (+ _coalesced, _into_tensor_coalesced,
+_allgather_base), reduce_scatter (+ _tensor_coalesced, _reduce_scatter_base), alltoall (lists) and alltoall_base, gather, scatter,
+send, recv, barrier and the coalescing hooks _start_coalescing / _end_coalescing, so also gather_object, scatter_object_list,
+all_gather_coalesced and _coalescing_manager.  The list forms of gather, scatter and alltoall take blocks of any size, zero
+included.  torch.bool tensors travel as uint8: SUM / MAX are logical or, PRODUCT / MIN logical and, AVG is refused.
+Not served, each with an error that names it: recv_anysource (on CUDA tensors a send / recv pair matches in post order, so a
+receive must name its source), monitored_barrier and split_group.
+
 Every collective works inside `torch.cuda.graph`.  Wrap the warm-up iterations and the capture in `pg.graphed()` (see
 Communicator.graphed) so that the captured collectives reuse the zero-copy tables their warm-up posts resolved."""
 from __future__ import annotations
+
+import itertools
 
 import torch
 import torch.distributed as dist
@@ -32,13 +42,37 @@ def _op(o):
     raise ValueError(f"unsupported reduce op {o}")
 
 
+def _flat(n, like):
+    """1-D buffer of `n` elements of `like`'s dtype and device, never at address 0, even when `n` is 0"""
+    return torch.empty(max(n, 1), dtype=like.dtype, device=like.device)[:n]
+
+
+def _views(flat, tensors):
+    """`flat` cut into consecutive views, one per tensor and shaped like it"""
+    offs = itertools.accumulate((t.numel() for t in tensors), initial=0)
+    return [flat[o:o + t.numel()].view(t.shape) for o, t in zip(offs, tensors)]
+
+
+def _pack(tensors):
+    flat = _flat(sum(t.numel() for t in tensors), tensors[0])
+    torch._foreach_copy_(_views(flat, tensors), list(tensors))
+    return flat
+
+
+def _displs(counts):
+    return list(itertools.accumulate(counts, initial=0))[:-1]
+
+
 class _Work(dist._Work):
-    def __init__(self, pg, reqs, result, cuda, side_stream=None):
+    def __init__(self, pg, reqs, result, cuda, side_stream=None, parts=()):
         super().__init__()
         self._pg, self._reqs, self._result, self._cuda = pg, reqs, result, cuda
         self._side = side_stream      # CUDA p2p runs on an internal stream; wait() makes the caller's stream wait for it
+        self._parts = parts           # the Work of every operation of a coalescing block
         self._fut = torch.futures.Future()
         self._done = False
+        if pg._coalesced is not None:
+            pg._coalesced.append(self)
 
     def _finish(self):
         if self._done:
@@ -51,11 +85,13 @@ class _Work(dist._Work):
             r.finalize_later() if self._cuda else r.finalize()
         if self._side is not None:
             torch.cuda.current_stream().wait_stream(self._side)
+        for w in self._parts:
+            w._finish()
         self._done = True
         self._fut.set_result(self._result)
 
     def is_completed(self):
-        return all(r.test() == 0 for r in self._reqs)
+        return all(r.test() == 0 for r in self._reqs) and all(w.is_completed() for w in self._parts)
 
     def is_success(self):
         return True
@@ -78,6 +114,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         self._comm = Communicator(store=store, rank=rank, size=size)
         self._pending = []   # CUDA requests whose kernels are in flight; finalized lazily
         self._p2p_streams = {}
+        self._coalesced = None   # between _start_coalescing and _end_coalescing: the Work of every operation
 
     def getBackendName(self):
         return "ucc_b200"
@@ -100,6 +137,15 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
                 r.post()
         self._reap()
         return _Work(self, reqs, result, cuda)
+
+    def _copy_out(self, w, outs, views):
+        """outs[i] <- views[i] once the collective of `w` has written the views: stream-ordered behind it on CUDA, after the wait
+        on the host"""
+        if not outs:
+            return
+        if not outs[0].is_cuda:
+            w.wait()
+        torch._foreach_copy_(outs, views)
 
     def _reap(self):
         keep = []
@@ -138,22 +184,19 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         return self._run(reqs, tensors, tensors)
 
     def allgather(self, output_lists, input_tensors, opts=None):
-        reqs, flats = [], []
-        for outs, inp in zip(output_lists, input_tensors):
-            flat = torch.empty((len(outs),) + tuple(inp.shape), dtype=inp.dtype, device=inp.device)
+        reqs, outs, views = [], [], []
+        for blocks, inp in zip(output_lists, input_tensors):
+            flat = torch.empty((len(blocks),) + tuple(inp.shape), dtype=inp.dtype, device=inp.device)
             reqs.append(self._comm.coll_init("allgather", inp.contiguous(), flat))
-            flats.append((flat, outs))
+            outs += blocks
+            views += list(flat)
         w = self._run(reqs, input_tensors, output_lists)
-        if input_tensors and input_tensors[0].is_cuda:
-            for flat, outs in flats:      # stream-ordered behind the collective
-                for i, o in enumerate(outs):
-                    o.copy_(flat[i])
-        else:
-            w.wait()
-            for flat, outs in flats:
-                for i, o in enumerate(outs):
-                    o.copy_(flat[i])
+        self._copy_out(w, outs, views)
         return w
+
+    def allgather_coalesced(self, output_lists, input_list, opts=None):
+        # output_lists[r][i] receives input_list[i] of rank r: one allgather per input
+        return self.allgather([list(blocks) for blocks in zip(*output_lists)], input_list, opts)
 
     def _allgather_base(self, output, input, opts=None):
         return self._run([self._comm.coll_init("allgather", input.contiguous(), output)], [input], output)
@@ -164,6 +207,10 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     def _reduce_scatter_base(self, output, input, opts=None):
         op = _op(opts.reduceOp) if opts is not None else "sum"
         return self._run([self._comm.coll_init("reduce_scatter", input.contiguous(), output, op=op)], [input], output)
+
+    def reduce_scatter_tensor_coalesced(self, outputs, inputs, opts=None):
+        op = _op(opts.reduceOp) if opts is not None else "sum"
+        return self._run([self._comm.coll_init("reduce_scatter", i.contiguous(), o, op=op) for o, i in zip(outputs, inputs)], inputs, outputs)
 
     def reduce_scatter(self, outputs, input_lists, opts=None):
         op = _op(opts.reduceOp) if opts is not None else "sum"
@@ -181,6 +228,69 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         equal = not output_split_sizes and not input_split_sizes
         req = _alltoall_init(self._comm, output, input.contiguous(), None if equal else output_split_sizes, None if equal else input_split_sizes)
         return self._run([req], [input], output)
+
+    # A rank cannot see the block sizes of the others (a gather's non-roots do not even see the root's list), so deciding between a
+    # collective and its V form by the local sizes could post ALLTOALL on one rank and ALLTOALLV on another - e.g. on a rank that
+    # moves nothing in this step - and the two do not match.  The list forms therefore always post the V form.
+    # Inside graphed() requests are cached by their buffers, and every member must create a new request or re-post a cached one in
+    # step with the others (tl/nvl matches the zero-copy exchange by post order).  The root's flat buffer of a gather or scatter is
+    # new on every call, so inside graphed() the other ranks move their block through a new buffer, too.
+    def alltoall(self, output_tensors, input_tensors, opts=None):
+        dst = _flat(sum(t.numel() for t in output_tensors), output_tensors[0])
+        req = _alltoall_init(self._comm, dst, _pack(input_tensors), [t.numel() for t in output_tensors], [t.numel() for t in input_tensors])
+        w = self._run([req], input_tensors, output_tensors)
+        self._copy_out(w, output_tensors, _views(dst, output_tensors))
+        return w
+
+    def gather(self, output_tensors, input_tensors, opts=None):
+        """the root passes one list of N blocks per input, the other ranks pass []"""
+        root = opts.rootRank if opts is not None else 0
+        reqs, outs, views = [], [], []
+        for i, inp in enumerate(input_tensors):
+            src = inp.contiguous() if inp.numel() and not self._comm._graphing else _pack([inp])
+            if self.rank() != root:
+                reqs.append(self._comm.coll_init("gatherv", src, None, root=root))
+                continue
+            blocks = output_tensors[i]
+            counts = [t.numel() for t in blocks]
+            flat = _flat(sum(counts), inp)
+            reqs.append(self._comm.coll_init("gatherv", src, flat, root=root, dst_counts=counts, dst_displs=_displs(counts)))
+            outs += blocks
+            views += _views(flat, blocks)
+        w = self._run(reqs, input_tensors, output_tensors)
+        self._copy_out(w, outs, views)
+        return w
+
+    def scatter(self, output_tensors, input_tensors, opts=None):
+        """the root passes one list of N blocks per output, the other ranks pass []"""
+        root = opts.rootRank if opts is not None else 0
+        reqs, outs, views = [], [], []
+        for i, out in enumerate(output_tensors):
+            dst = out
+            if not out.numel() or self._comm._graphing:
+                dst = _flat(out.numel(), out)
+                outs.append(out)
+                views.append(dst.view(out.shape))
+            if self.rank() != root:
+                reqs.append(self._comm.coll_init("scatterv", None, dst, root=root))
+                continue
+            counts = [t.numel() for t in input_tensors[i]]
+            reqs.append(self._comm.coll_init("scatterv", _pack(input_tensors[i]), dst, root=root, src_counts=counts, src_displs=_displs(counts)))
+        w = self._run(reqs, output_tensors, output_tensors)
+        self._copy_out(w, outs, views)
+        return w
+
+    # ---- coalescing (torch's _coalescing_manager with a device): one Work that completes every operation of the block
+    def _start_coalescing(self, device):
+        if self._coalesced is not None:
+            raise RuntimeError("ucc_b200: _start_coalescing while a coalescing block is already open")
+        self._coalesced = []
+
+    def _end_coalescing(self, device):
+        if self._coalesced is None:
+            raise RuntimeError("ucc_b200: _end_coalescing without _start_coalescing")
+        works, self._coalesced = self._coalesced, None
+        return _Work(self, [], None, False, parts=works)
 
     # ---- point to point: a two-member active-set broadcast, exactly how ProcessGroupUCC maps send/recv onto UCC.
     # CUDA tensors travel over tl/nvl's heap channels: messages between an ordered pair of ranks are matched in POST ORDER (the NCCL
@@ -212,10 +322,20 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     def recv(self, tensors, srcRank, tag=0):
         return self._p2p(tensors, srcRank, self.rank(), tag)
 
+    def recv_anysource(self, tensors, tag=0):
+        raise RuntimeError("ucc_b200 does not support recv_anysource: send / recv pairs match in post order on CUDA tensors, so "
+                           "every receive must name its source")
+
     def barrier(self, opts=None):
         self._comm.barrier()
         w = _Work(self, [], None, False)
         return w
+
+    def monitored_barrier(self, *args, **kwargs):
+        raise RuntimeError("ucc_b200 does not support monitored_barrier: use barrier")
+
+    def split_group(self, *args, **kwargs):
+        raise RuntimeError("ucc_b200 does not support split_group")
 
     def shutdown(self):
         for r in self._pending:
