@@ -7,16 +7,24 @@
     torch.nn.parallel.DistributedDataParallel(model)   # gradient buckets go through the same path
 
 The process group is a Python subclass of `torch.distributed.ProcessGroup`; wire-up uses the rendezvous store as the
-UCC out-of-band allgather.  CUDA collectives are posted stream-ordered on the caller's current stream, so `Work.wait()`
-only has to make sure the kernel is in the stream (it does not block the host on the GPU).
+UCC out-of-band allgather.  Every group it makes (the default group, `new_group` groups, DeviceMesh dimension groups) keeps
+the name and description torch gives it, so PyTorch's own parallel stack runs on it: `_functional_collectives` (also under
+`torch.compile`, whose `_c10d_functional` ops find the group by that name), DeviceMesh, DTensor, FSDP2 (`fully_shard`, HSDP)
+and `torch.distributed.tensor.parallel`.
+
+CUDA collectives are posted stream-ordered on the caller's current stream; the host does not wait for the GPU.  `Work.wait()`
+makes sure the kernels are in that stream and then makes the stream current at wait() wait for them, as ProcessGroupNCCL's does:
+a collective posted on a side stream and waited for on another is read there only after it has run.
 
 c10d operations served: allreduce (+ _coalesced), broadcast, reduce, allgather (+ _coalesced, _into_tensor_coalesced,
 _allgather_base), reduce_scatter (+ _tensor_coalesced, _reduce_scatter_base), alltoall (lists) and alltoall_base, gather, scatter,
 send, recv, barrier and the coalescing hooks _start_coalescing / _end_coalescing, so also gather_object, scatter_object_list,
-all_gather_coalesced and _coalescing_manager.  The list forms of gather, scatter and alltoall take blocks of any size, zero
-included.  torch.bool tensors travel as uint8: SUM / MAX are logical or, PRODUCT / MIN logical and, AVG is refused.
-Not served, each with an error that names it: recv_anysource (on CUDA tensors a send / recv pair matches in post order, so a
-receive must name its source), monitored_barrier and split_group.
+all_gather_coalesced and _coalescing_manager.  The list forms of allgather, reduce_scatter, gather, scatter and alltoall take
+blocks of any size, zero included.  torch.bool tensors travel as uint8: SUM / MAX are logical or, PRODUCT / MIN logical and, AVG
+is refused.
+Not served, each with an error that names it: ReduceOp.PREMUL_SUM (its factor cannot be read from Python and the library has no
+scaled sum; FSDP2 uses it only for a custom gradient divide factor), recv_anysource (on CUDA tensors a send / recv pair matches in
+post order, so a receive must name its source), monitored_barrier and split_group.
 
 Every collective works inside `torch.cuda.graph`.  Wrap the warm-up iterations and the capture in `pg.graphed()` (see
 Communicator.graphed) so that the captured collectives reuse the zero-copy tables their warm-up posts resolved."""
@@ -39,6 +47,9 @@ def _op(o):
     for k, v in _OPS.items():
         if o == k:
             return v
+    if o == dist.ReduceOp.PREMUL_SUM:
+        # the factor of a PREMUL_SUM op cannot be read from Python, and the library has no scaled sum
+        raise ValueError("ucc_b200 does not support ReduceOp.PREMUL_SUM: use SUM or AVG and scale the tensor")
     raise ValueError(f"unsupported reduce op {o}")
 
 
@@ -64,10 +75,11 @@ def _displs(counts):
 
 
 class _Work(dist._Work):
-    def __init__(self, pg, reqs, result, cuda, side_stream=None, parts=()):
+    def __init__(self, pg, reqs, result, cuda, side_stream=None, parts=(), posted=None):
         super().__init__()
         self._pg, self._reqs, self._result, self._cuda = pg, reqs, result, cuda
         self._side = side_stream      # CUDA p2p runs on an internal stream; wait() makes the caller's stream wait for it
+        self._posted = posted         # CUDA collectives: (stream, event recorded on it behind the collective's kernels)
         self._parts = parts           # the Work of every operation of a coalescing block
         self._fut = torch.futures.Future()
         self._done = False
@@ -85,6 +97,13 @@ class _Work(dist._Work):
             r.finalize_later() if self._cuda else r.finalize()
         if self._side is not None:
             torch.cuda.current_stream().wait_stream(self._side)
+        if self._posted is not None:
+            # c10d contract (ProcessGroupNCCL's WorkNCCL::wait): work the caller queues after wait() on its current stream runs
+            # after the collective, also when it was posted on another stream.  The host does not wait.
+            stream, event = self._posted
+            current = torch.cuda.current_stream()
+            if current != stream:
+                current.wait_event(event)
         for w in self._parts:
             w._finish()
         self._done = True
@@ -115,9 +134,29 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         self._pending = []   # CUDA requests whose kernels are in flight; finalized lazily
         self._p2p_streams = {}
         self._coalesced = None   # between _start_coalescing and _end_coalescing: the Work of every operation
+        self._name, self._desc = None, None
 
     def getBackendName(self):
         return "ucc_b200"
+
+    # torch uses this object as the group itself, with no c10d Backend registered inside it, and ProcessGroup keeps its name and
+    # description in such a Backend.  Keep them here instead: _functional_collectives, DeviceMesh, DTensor and FSDP2 find the group
+    # by its name (the _c10d_functional ops resolve the name torch registered with this object and call back into it).
+    def _set_group_name(self, name):
+        self._name = name
+
+    @property
+    def group_name(self):
+        if self._name is None:
+            raise RuntimeError("ucc_b200: the process group has no name yet")
+        return self._name
+
+    def _set_group_desc(self, desc):
+        self._desc = desc
+
+    @property
+    def group_desc(self):
+        return self._desc if self._desc is not None else "undefined"
 
     def graphed(self):
         """context manager for the warm-up and the capture of a CUDA graph: Communicator.graphed() of this group"""
@@ -127,7 +166,9 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         self._comm.release_graphed()
 
     # ---- helpers
-    def _run(self, reqs, tensors, result, wait_posted=True):
+    def _run(self, reqs, tensors, result, wait_posted=True, outs=(), views=()):
+        """post `reqs`; then outs[i] <- views[i] once the collectives have written the views: stream-ordered behind them on CUDA,
+        after the wait on the host"""
         cuda = bool(tensors) and tensors[0].is_cuda
         for r in reqs:
             if cuda:
@@ -135,17 +176,19 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
                 r.finalize_later = lambda r=r: self._pending.append(r)
             else:
                 r.post()
+        posted = None
+        if cuda:
+            if outs:
+                torch._foreach_copy_(outs, views)
+            if wait_posted:   # every kernel is in the stream, a deferred zero-copy launch included: mark the stream behind them
+                stream = torch.cuda.current_stream()
+                posted = (stream, stream.record_event())
         self._reap()
-        return _Work(self, reqs, result, cuda)
-
-    def _copy_out(self, w, outs, views):
-        """outs[i] <- views[i] once the collective of `w` has written the views: stream-ordered behind it on CUDA, after the wait
-        on the host"""
-        if not outs:
-            return
-        if not outs[0].is_cuda:
+        w = _Work(self, reqs, result, cuda, posted=posted)
+        if outs and not cuda:
             w.wait()
-        torch._foreach_copy_(outs, views)
+            torch._foreach_copy_(outs, views)
+        return w
 
     def _reap(self):
         keep = []
@@ -183,16 +226,24 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         reqs = [self._comm.coll_init("reduce", None if me == root else t, t if me == root else None, op=op, root=root, inplace=me == root) for t in tensors]
         return self._run(reqs, tensors, tensors)
 
+    # The list forms of allgather and reduce_scatter hold one block per rank, and every rank passes the whole list, so every rank
+    # sees every block size.  Blocks of one size post ALLGATHER / REDUCE_SCATTER, blocks of different sizes (zero included) post
+    # ALLGATHERV / REDUCE_SCATTERV, and all ranks make the same choice.
     def allgather(self, output_lists, input_tensors, opts=None):
         reqs, outs, views = [], [], []
         for blocks, inp in zip(output_lists, input_tensors):
-            flat = torch.empty((len(blocks),) + tuple(inp.shape), dtype=inp.dtype, device=inp.device)
-            reqs.append(self._comm.coll_init("allgather", inp.contiguous(), flat))
+            counts = [t.numel() for t in blocks]
+            if len(set(counts)) == 1:
+                flat = torch.empty((len(blocks),) + tuple(inp.shape), dtype=inp.dtype, device=inp.device)
+                reqs.append(self._comm.coll_init("allgather", inp.contiguous(), flat))
+                views += list(flat)
+            else:
+                flat = _flat(sum(counts), inp)
+                src = inp.contiguous() if inp.numel() else _pack([inp])
+                reqs.append(self._comm.coll_init("allgatherv", src, flat, dst_counts=counts, dst_displs=_displs(counts)))
+                views += _views(flat, blocks)
             outs += blocks
-            views += list(flat)
-        w = self._run(reqs, input_tensors, output_lists)
-        self._copy_out(w, outs, views)
-        return w
+        return self._run(reqs, input_tensors, output_lists, outs=outs, views=views)
 
     def allgather_coalesced(self, output_lists, input_list, opts=None):
         # output_lists[r][i] receives input_list[i] of rank r: one allgather per input
@@ -216,9 +267,15 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         op = _op(opts.reduceOp) if opts is not None else "sum"
         reqs, keep = [], []
         for out, ins in zip(outputs, input_lists):
-            flat = torch.cat([t.reshape(-1) for t in ins])
+            counts = [t.numel() for t in ins]
+            if len(set(counts)) == 1:
+                flat = torch.cat([t.reshape(-1) for t in ins])
+                reqs.append(self._comm.coll_init("reduce_scatter", flat, out, op=op))
+            else:
+                flat = _pack(ins)
+                dst = out if out.numel() else _flat(0, out)
+                reqs.append(self._comm.coll_init("reduce_scatterv", flat, dst, op=op, dst_counts=counts, dst_displs=_displs(counts)))
             keep.append(flat)
-            reqs.append(self._comm.coll_init("reduce_scatter", flat, out, op=op))
         w = self._run(reqs, outputs, outputs)
         w._keep = keep
         return w
@@ -231,16 +288,15 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     # A rank cannot see the block sizes of the others (a gather's non-roots do not even see the root's list), so deciding between a
     # collective and its V form by the local sizes could post ALLTOALL on one rank and ALLTOALLV on another - e.g. on a rank that
-    # moves nothing in this step - and the two do not match.  The list forms therefore always post the V form.
+    # moves nothing in this step - and the two do not match.  The list forms of alltoall, gather and scatter therefore always post
+    # the V form.
     # Inside graphed() requests are cached by their buffers, and every member must create a new request or re-post a cached one in
     # step with the others (tl/nvl matches the zero-copy exchange by post order).  The root's flat buffer of a gather or scatter is
     # new on every call, so inside graphed() the other ranks move their block through a new buffer, too.
     def alltoall(self, output_tensors, input_tensors, opts=None):
         dst = _flat(sum(t.numel() for t in output_tensors), output_tensors[0])
         req = _alltoall_init(self._comm, dst, _pack(input_tensors), [t.numel() for t in output_tensors], [t.numel() for t in input_tensors])
-        w = self._run([req], input_tensors, output_tensors)
-        self._copy_out(w, output_tensors, _views(dst, output_tensors))
-        return w
+        return self._run([req], input_tensors, output_tensors, outs=output_tensors, views=_views(dst, output_tensors))
 
     def gather(self, output_tensors, input_tensors, opts=None):
         """the root passes one list of N blocks per input, the other ranks pass []"""
@@ -257,9 +313,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
             reqs.append(self._comm.coll_init("gatherv", src, flat, root=root, dst_counts=counts, dst_displs=_displs(counts)))
             outs += blocks
             views += _views(flat, blocks)
-        w = self._run(reqs, input_tensors, output_tensors)
-        self._copy_out(w, outs, views)
-        return w
+        return self._run(reqs, input_tensors, output_tensors, outs=outs, views=views)
 
     def scatter(self, output_tensors, input_tensors, opts=None):
         """the root passes one list of N blocks per output, the other ranks pass []"""
@@ -276,9 +330,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
                 continue
             counts = [t.numel() for t in input_tensors[i]]
             reqs.append(self._comm.coll_init("scatterv", _pack(input_tensors[i]), dst, root=root, src_counts=counts, src_displs=_displs(counts)))
-        w = self._run(reqs, output_tensors, output_tensors)
-        self._copy_out(w, outs, views)
-        return w
+        return self._run(reqs, output_tensors, output_tensors, outs=outs, views=views)
 
     # ---- coalescing (torch's _coalescing_manager with a device): one Work that completes every operation of the block
     def _start_coalescing(self, device):
