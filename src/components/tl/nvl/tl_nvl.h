@@ -207,7 +207,8 @@ typedef enum { NVL_TASK_LAUNCHED, NVL_TASK_QUEUED, NVL_TASK_P2P_WAIT /* send wai
  * from registrations at init, the tables the first post of a persistent request resolved, or the exchange board at every post.
  * It holds no pointer into the task: nvl_rebuild swaps task bodies. */
 enum { NVL_ZC_SRC = 1, NVL_ZC_DST = 2, /* sides every member's direct form touches */
-       NVL_ZC_ALIGN = 4 /* a board entry that is not 16-byte aligned makes every member stage */ };
+       NVL_ZC_ALIGN = 4, /* a board entry that is not 16-byte aligned makes every member stage */
+       NVL_ZC_WITHDRAW = 8 /* I publish my buffers as not mappable, which makes every member stage */ };
 typedef enum { NVL_ZC_RESOLVE, NVL_ZC_STAGED, NVL_ZC_DIRECT } nvl_zc_cache_t;
 typedef struct nvl_zc {
     unsigned       flags;              /* NVL_ZC_*; 0: the direct form is not wanted */
@@ -262,6 +263,7 @@ ucc_status_t ucc_tl_nvl_xb_create(ucc_tl_nvl_team_t *team);
 ucc_status_t ucc_tl_nvl_xb_attach(ucc_tl_nvl_team_t *team);
 void         ucc_tl_nvl_xb_unlink(ucc_tl_nvl_team_t *team);
 void         ucc_tl_nvl_xb_release(ucc_tl_nvl_team_t *team);
+int          ucc_tl_nvl_is_managed(const void *ptr);
 void         ucc_tl_nvl_xb_export(ucc_tl_nvl_team_t *team, const void *ptr, size_t len, nvl_xb_buf_t *b);
 char        *ucc_tl_nvl_xb_import(ucc_tl_nvl_team_t *team, ucc_rank_t p, const nvl_xb_buf_t *b);
 void         ucc_tl_nvl_zc_init(ucc_tl_nvl_team_t *team, nvl_zc_t *zc, unsigned flags, const void *src, size_t src_len, void *dst, size_t dst_len, const ucc_coll_args_t *reg);

@@ -31,7 +31,10 @@ static int to_nvl_op(ucc_reduction_op_t op)
     default: return -1;
     }
 }
-static inline int is_cuda(ucc_memory_type_t mt) { return mt == UCC_MEMORY_TYPE_CUDA; }
+/* device or managed memory: the kernels read the local source and write the local destination with ordinary global loads and
+ * stores, which are correct for managed pages wherever they live.  A managed buffer is never mapped by a peer (tl_nvl_direct.c:
+ * export_buf), so its collectives run the staged forms. */
+static inline int is_cuda(ucc_memory_type_t mt) { return mt == UCC_MEMORY_TYPE_CUDA || mt == UCC_MEMORY_TYPE_CUDA_MANAGED; }
 
 /* ------------------------------------------------------------------ */
 /* task life cycle                                                     */
@@ -605,8 +608,10 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
      * limit, medians of 7 rounds of 20 copies): 1 GiB 709.8 us, against 713.8 us for the best kernel candidate (non-persistent
      * TMA ring, 16 KB x 4 stages, 4 chunks per CTA), 715.5 us for the best thread copy and 732.3 us for the former persistent
      * TMA ring; 64 MB 47.7 us against 49.7 us for the thread copy below; 16 MB 8.9 us against 11.1 us.  Smaller copies, not
-     * measured against it, keep the thread copy. */
-    st = task_alloc(b, b_team, copy >= ((size_t)16 << 20) ? NVL_PATH_SELF_COPY_CE : NVL_PATH_SELF_COPY, &t);
+     * measured against it, keep the thread copy.  A managed side always takes the thread copy, as a precaution (cudaMemcpyAsync on
+     * managed pages was not measured): the kernel's loads and stores are correct for its pages wherever they live, where
+     * cudaMemcpyAsync would be handed a device-to-device kind for them. */
+    st = task_alloc(b, b_team, copy >= ((size_t)16 << 20) && smt == UCC_MEMORY_TYPE_CUDA && dmt == UCC_MEMORY_TYPE_CUDA ? NVL_PATH_SELF_COPY_CE : NVL_PATH_SELF_COPY, &t);
     if (st != UCC_OK) return st;
     memset(&t->u.xchg, 0, sizeof(t->u.xchg));
     t->u.xchg.src = src; t->u.xchg.dst = dst; t->u.xchg.src_bytes = copy;
@@ -959,6 +964,10 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
             if (x.dst_off[p] + x.pull_bytes[p] > dst_len) dst_len = x.dst_off[p] + x.pull_bytes[p];
         }
         ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, x.dst, dst_len, NULL);
+        /* the direct forms of bulk and ce hand my source to the TMA engine or the copy engines.  As a precaution (not measured on
+         * managed pages) a managed source withdraws my destination there, and every member runs the staged pull; the thread push
+         * reads my source with ordinary loads and keeps its direct form */
+        if (t->zc.flags && (path == NVL_PATH_PUSH_BULK || path == NVL_PATH_PUSH_CE) && ucc_tl_nvl_is_managed(x.src)) t->zc.flags |= NVL_ZC_WITHDRAW;
     }
     *task_p = &t->super;
     return UCC_OK;
@@ -1055,12 +1064,13 @@ ucc_status_t ucc_tl_nvl_team_get_scores(ucc_base_team_t *b_team, ucc_coll_score_
 {
     ucc_tl_nvl_team_t *team = ucc_derived_of(b_team, ucc_tl_nvl_team_t);
     ucc_tl_nvl_context_t *ctx = NVL_CTX(team);
-    ucc_memory_type_t mt[1] = {UCC_MEMORY_TYPE_CUDA};
-    ucc_coll_score_team_info_t info = {UCC_TL_NVL_DEFAULT_SCORE, UCC_TL_TEAM_SIZE(team), UCC_TL_NVL_SUPPORTED_COLLS, mt, 1, ucc_tl_nvl_coll_init, ucc_tl_nvl_alg_id_to_init};
+    /* managed buffers get the same ranges and scores as device buffers: they run the same kernels, staged */
+    ucc_memory_type_t mt[2] = {UCC_MEMORY_TYPE_CUDA, UCC_MEMORY_TYPE_CUDA_MANAGED};
+    ucc_coll_score_team_info_t info = {UCC_TL_NVL_DEFAULT_SCORE, UCC_TL_TEAM_SIZE(team), UCC_TL_NVL_SUPPORTED_COLLS, mt, 2, ucc_tl_nvl_coll_init, ucc_tl_nvl_alg_id_to_init};
     ucc_coll_score_t *score;
     char sel[512], a[32], n[32];
     /* a team of one outranks tl/self (50) for CUDA buffers: its copy is a stream-ordered kernel instead of a blocking memcpy */
-    ucc_status_t st = ucc_coll_score_build_default(b_team, team->self ? 60 : UCC_TL_NVL_DEFAULT_SCORE, ucc_tl_nvl_coll_init, UCC_TL_NVL_SUPPORTED_COLLS, mt, 1, &score);
+    ucc_status_t st = ucc_coll_score_build_default(b_team, team->self ? 60 : UCC_TL_NVL_DEFAULT_SCORE, ucc_tl_nvl_coll_init, UCC_TL_NVL_SUPPORTED_COLLS, mt, 2, &score);
     if (st != UCC_OK) return st;
     if (team->self) { info.default_score = 60; st = ucc_tl_apply_tune(&team->super, score, &info, NULL, ctx->cfg.super.super.score_str); if (st != UCC_OK) { ucc_coll_score_free(score); return st; } *score_p = score; return UCC_OK; }
     snprintf(a, sizeof(a), "%zu", ctx->cfg.oneshot_thresh + 1); /* ranges are end-exclusive, the threshold itself is still one-shot */

@@ -83,11 +83,23 @@ void ucc_tl_nvl_xb_release(ucc_tl_nvl_team_t *team)
     if (team->xb_mine) { ucc_shm_detach(team->xb_mine, sizeof(nvl_xb_seg_t)); team->xb_mine = NULL; }
 }
 
+int ucc_tl_nvl_is_managed(const void *ptr)
+{
+    struct cudaPointerAttributes attr;
+    if (!ptr) return 0;
+    if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
+    return attr.type == cudaMemoryTypeManaged;
+}
+
+/* A managed buffer (cudaMallocManaged) is never published as mappable, whatever the sharing mode: a peer GPU that loads or stores
+ * its pages migrates them or takes a remote fault on every access, so every member stages the collective instead.  Across processes
+ * cudaIpcGetMemHandle refuses such memory anyway; inside one process the board would carry the raw pointer. */
 static void export_buf(ucc_tl_nvl_team_t *team, const void *ptr, size_t len, nvl_xb_buf_t *b)
 {
     memset(b, 0, sizeof(*b));
     if (!ptr || !len) { b->kind = NVL_XB_EMPTY; return; }
     b->len = len;
+    if (ucc_tl_nvl_is_managed(ptr)) { b->kind = NVL_XB_NONE; return; }
     if (team->heap_kind == NVL_HEAP_LOCAL) { b->kind = NVL_XB_RAW; b->base = (uint64_t)(uintptr_t)ptr; return; }
     {
         void *base = NULL; size_t alen = 0;
@@ -106,7 +118,7 @@ static int xb_publish(ucc_tl_nvl_team_t *team, const nvl_zc_t *zc, int usable, c
     nvl_xb_entry_t *e = &team->xb_mine->e[zc->seq % NVL_XB_SLOTS];
     if (zc->seq >= NVL_XB_SLOTS)
         for (ucc_rank_t p = 0; p < N; p++) if (p != me && ucc_load_acquire(&team->xb[p]->consumed) + NVL_XB_SLOTS <= zc->seq) return 0;
-    if (usable) { export_buf(team, zc->src, zc->src_len, &e->src); export_buf(team, zc->dst, zc->dst_len, &e->dst); }
+    if (usable && !(zc->flags & NVL_ZC_WITHDRAW)) { export_buf(team, zc->src, zc->src_len, &e->src); export_buf(team, zc->dst, zc->dst_len, &e->dst); }
     else { memset(&e->src, 0, sizeof(e->src)); memset(&e->dst, 0, sizeof(e->dst)); e->src.kind = e->dst.kind = NVL_XB_NONE; }
     for (ucc_rank_t p = 0; p < N && p < NVL_MAX_PEERS; p++) e->aux[p] = aux ? (uint64_t)aux[p] : 0;
     ucc_store_release(&e->seq, zc->seq + 1);

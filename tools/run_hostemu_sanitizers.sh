@@ -4,7 +4,7 @@
 # launch queue, exchange board, ...) cannot be sanitised on a GPU box without the CUDA runtime getting in the way; against the
 # emulated runtime it can.
 # A run is a scenario of tests/hostemu_worker.py, or worker:scenario for tests/hostemu_<worker>_worker.py (e.g. graph:graphs,
-# int128:zcopy); every run uses the one plugin of tests/emu/build_hostemu.sh.
+# int128:zcopy, managed:all); every run uses the one plugin of tests/emu/build_hostemu.sh.
 cd "$(dirname "$0")/.."
 export EMU_CC=/usr/bin/gcc EMU_CXX=/usr/bin/g++
 rc=0
@@ -13,7 +13,7 @@ for san in thread address; do
   rm -f /tmp/ucc_b200_he_$san.*
   lib=$(/usr/bin/gcc -print-file-name=$([ $san = thread ] && echo libtsan.so || echo libasan.so))
   for s in ${HOSTEMU_SCENARIOS:-allreduce colls_staged colls_zcopy colls_push colls_ce misc triggered p2p memh lanes complex: \
-                                swap:zcopy swap:staged swap:persistent swap:memh swap:big_team swap:tune}; do
+                                swap:zcopy swap:staged swap:persistent swap:memh swap:big_team swap:tune managed:all}; do
     case $s in *:*) worker=tests/hostemu_${s%%:*}_worker.py;; *) worker=tests/hostemu_worker.py;; esac
     log=/tmp/ucc_b200_he_${san}_${s/:/_}.log
     LD_PRELOAD=$lib TSAN_OPTIONS="log_path=/tmp/ucc_b200_he_$san:halt_on_error=0:report_signal_unsafe=0" \

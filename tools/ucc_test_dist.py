@@ -49,12 +49,41 @@ def is_float(dt):
     return dt in ("float16", "float32", "float64", "bfloat16")
 
 
+_MANAGED = []   # headers of the managed allocations
+
+
+def release_managed():
+    """free the managed buffers of the cases run so far (while the library, and with it the memory component, is alive)"""
+    if _MANAGED:
+        torch.cuda.synchronize()
+        for h in _MANAGED:
+            st = U.lib.ucc_mc_free(h)
+            assert st == U.UCC_OK, f"ucc_mc_free: {U.status_str(st)}"
+        _MANAGED.clear()
+
+
+class _Cai:
+    def __init__(self, ptr, nbytes):
+        self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 3}
+
+
 class Buf:
     """`count` elements of `dt` in host or CUDA memory; contents move as logical float64/int64 numpy arrays"""
 
     def __init__(self, dt, count, mtype):
         self.dt, self.count, self.mtype = dt, count, mtype
-        self.t = torch.zeros(max(count, 1) * dt_size(dt), dtype=torch.uint8, device="cuda" if mtype == "cuda" else "cpu")
+        nbytes = max(count, 1) * dt_size(dt)
+        if mtype == "cudaManaged":
+            # cudaMallocManaged through the library's memory component, viewed as a CUDA tensor (no copy); freed after the batch that used it
+            hdr = C.c_void_p()
+            assert U.lib.ucc_mc_alloc(C.byref(hdr), nbytes, MEM[mtype]) == U.UCC_OK
+            _MANAGED.append(hdr)
+            ptr = C.c_void_p.from_address(hdr.value + 8).value     # ucc_mc_buffer_header_t: {int mt; int from_pool; void *addr}
+            self.t = torch.as_tensor(_Cai(ptr, nbytes), device="cuda")
+            self.t.zero_()
+            self.settle()
+        else:
+            self.t = torch.zeros(nbytes, dtype=torch.uint8, device="cuda" if mtype == "cuda" else "cpu")
 
     def reset(self):
         """back to the initial contents (persistent collectives are posted several times, in-place ones consume their input)"""
@@ -62,6 +91,14 @@ class Buf:
             self.set(self.init)
         else:
             self.t.zero_()
+            self.settle()
+
+    def settle(self):
+        """managed buffers: wait for the writes queued on torch's stream.  A plain post runs on the library's own non-blocking
+        stream, unordered with them, and a first touch of managed pages migrates them, so these writes can still be running when the
+        collective starts"""
+        if self.mtype == "cudaManaged":
+            torch.cuda.current_stream().synchronize()
 
     @property
     def ptr(self):
@@ -78,6 +115,7 @@ class Buf:
         else:
             raw = torch.from_numpy(vals.astype(NP_DT[self.dt]).view(np.uint8).copy())
         self.t[:raw.numel()].copy_(raw)
+        self.settle()
 
     def get(self):
         raw = self.t[:self.count * dt_size(self.dt)].cpu()
@@ -399,7 +437,7 @@ def parse_args(argv):
     ap.add_argument("-Z", "--max_size", type=int, default=1 << 30, help="cases whose largest buffer exceeds this are skipped")
     ap.add_argument("-N", "--num_tests", type=int, default=1, help="number of tests to run in parallel (outstanding on the same team)")
     ap.add_argument("-i", "--iter", type=int, default=1)
-    ap.add_argument("--triggered", type=int, default=0, help="0 - post, 1 - triggered post (CUDA memory), 2 - both")
+    ap.add_argument("--triggered", type=int, default=0, help="0 - post, 1 - triggered post (CUDA or managed memory), 2 - both")
     ap.add_argument("-v", "--verbose", action="store_true")
     return ap.parse_args(argv)
 
@@ -412,7 +450,9 @@ def main(argv=None):
         if c not in ALL_COLLS:
             raise SystemExit(f"incorrect coll type: {c}")
     mtypes = a.mtypes.split(",")
-    use_cuda = "cuda" in mtypes
+    use_cuda = "cuda" in mtypes or "cudaManaged" in mtypes
+    U.lib.ucc_mc_alloc.argtypes = [C.POINTER(C.c_void_p), C.c_size_t, C.c_int]
+    U.lib.ucc_mc_free.argtypes = [C.c_void_p]
     rank, world, _ = init_distributed("cpu:gloo,cuda:nccl" if use_cuda else "gloo")
     if a.seed is None:
         s = torch.tensor([int(time.time()) & 0x7fffffff])
@@ -469,6 +509,7 @@ def main(argv=None):
                 if a.verbose and rank == 0:
                     print(f"[{'OK' if worst == 0 else 'SKIP' if worst == 1 else 'FAIL'}] {c['name']}", flush=True)
             batch.clear()
+            release_managed()
         for coll in colls:
             dts = ["int32"] if coll in NO_DATA else a.dtypes.split(",")
             ops = a.ops.split(",") if coll in REDUCTIONS else ["sum"]
@@ -480,12 +521,12 @@ def main(argv=None):
                     raise SystemExit(f"incorrect dtype/mtype: {dt}/{mtype}")
                 if coll in REDUCTIONS and op not in (FLOAT_OPS if is_float(dt) else INT_OPS):
                     continue
-                if trig and mtype != "cuda":
+                if trig and mtype == "host":
                     continue
                 count = max(size // dt_size(dt), 1) if coll not in NO_DATA else 0
                 name = f"{kind}/{coll}/{mtype}/{dt}/{op}/count={count}/root={root}/inplace={int(inplace)}/persistent={int(persistent)}/triggered={int(trig)}"
                 totals[0] += 1
-                if count * dt_size(dt) * (n if coll not in ("allreduce", "reduce", "bcast") else 1) > a.max_size or mtype == "cudaManaged":
+                if count * dt_size(dt) * (n if coll not in ("allreduce", "reduce", "bcast") else 1) > a.max_size:
                     totals[2] += 1
                     continue
                 built = build_case(coll, team, urank, n, a.seed, case, dt, op, mtype, count, root, inplace)
@@ -493,7 +534,7 @@ def main(argv=None):
                     totals[2] += 1
                     continue
                 batch.append({"name": name, "args": built[0], "check": built[1], "persistent": persistent, "triggered": trig,
-                              "cuda": mtype == "cuda"})
+                              "cuda": mtype != "host"})
                 if len(batch) >= max(a.num_tests, 1):
                     flush(batch)
         flush(batch)
