@@ -33,6 +33,16 @@ typedef enum {
 #define UCC_EEE_TASK_FLAG_REDUCE_WITH_ALPHA UCC_BIT(0)
 #define UCC_EEE_TASK_FLAG_REDUCE_SRCS_EXT   UCC_BIT(1)
 
+/* AVG passes alpha = 1.0 / n for the n contributions it averages.  Returns that n when alpha is exactly 1.0 / n for an integer
+ * n >= 1, else 0.  Integer types divide the sum by n (truncating): scaling by alpha in double drops the low bits of sums above 2^53. */
+static inline int ucc_ec_avg_divisor(double alpha)
+{
+    int n;
+    if (!(alpha > 0.0 && alpha <= 1.0) || 1.0 / alpha > 2147483647.0) return 0;
+    n = (int)(1.0 / alpha + 0.5);
+    return 1.0 / (double)n == alpha ? n : 0;
+}
+
 typedef struct ucc_ee_executor_params { uint64_t mask; ucc_ee_type_t ee_type; uint64_t task_types; } ucc_ee_executor_params_t;
 enum { UCC_EE_EXECUTOR_PARAM_FIELD_TYPE = UCC_BIT(0), UCC_EE_EXECUTOR_PARAM_FIELD_TASK_TYPES = UCC_BIT(1) };
 typedef struct ucc_ee_executor { ucc_ee_type_t ee_type; void *ee_context; } ucc_ee_executor_t;

@@ -184,19 +184,21 @@ static int describe(const ucc_ee_executor_task_args_t *a, ec_ring_slot_t *d)
         if (a->reduce.n_srcs > EC_MAX_SRCS) return -1;
         r->dst = a->reduce.dst; for (int i = 0; i < a->reduce.n_srcs; i++) r->srcs[i] = srcs[i];
         r->n_srcs = a->reduce.n_srcs; r->count = a->reduce.count; r->dt = to_ec_dt(a->reduce.dt); r->op = ec_op_index(a->reduce.op); r->with_alpha = with_alpha; r->alpha = a->reduce.alpha;
+        r->avg_n = with_alpha ? ucc_ec_avg_divisor(r->alpha) : 0;
         if (r->dt < 0 || r->op < 0 || !ec_dt_supports_op(r->dt, r->op) || (a->reduce.op == UCC_OP_AVG && !with_alpha)) return -1;
         return EC_TASK_REDUCE; }
     case UCC_EE_EXECUTOR_TASK_REDUCE_STRIDED: {
         ec_reduce_args_t *r = &d->u.reduce; memset(r, 0, sizeof(*r));
         r->dst = a->reduce_strided.dst; r->srcs[0] = a->reduce_strided.src1; r->src2 = a->reduce_strided.src2; r->stride = a->reduce_strided.stride; r->strided = 1;
         r->n_srcs = a->reduce_strided.n_src2 + 1; r->count = a->reduce_strided.count; r->dt = to_ec_dt(a->reduce_strided.dt); r->op = ec_op_index(a->reduce_strided.op);
-        r->with_alpha = with_alpha; r->alpha = a->reduce_strided.alpha;
-        if (r->dt < 0 || r->op < 0 || !ec_dt_supports_op(r->dt, r->op)) return -1;
+        r->with_alpha = with_alpha; r->alpha = a->reduce_strided.alpha; r->avg_n = with_alpha ? ucc_ec_avg_divisor(r->alpha) : 0;
+        if (r->dt < 0 || r->op < 0 || !ec_dt_supports_op(r->dt, r->op) || (a->reduce_strided.op == UCC_OP_AVG && !with_alpha)) return -1;
         return EC_TASK_REDUCE; }
     case UCC_EE_EXECUTOR_TASK_REDUCE_MULTI_DST: {
         ec_reduce_multi_dst_args_t *m = &d->u.rmd; memset(m, 0, sizeof(*m));
         m->n_bufs = a->reduce_multi_dst.n_bufs; m->dt = to_ec_dt(a->reduce_multi_dst.dt); m->op = ec_op_index(a->reduce_multi_dst.op);
-        if (m->n_bufs > EC_MULTI_BUFS || m->dt < 0 || m->op < 0 || !ec_dt_supports_op(m->dt, m->op)) return -1;
+        /* (AVG: the task has no alpha to scale by, so it would silently be a SUM) */
+        if (m->n_bufs > EC_MULTI_BUFS || m->dt < 0 || m->op < 0 || !ec_dt_supports_op(m->dt, m->op) || a->reduce_multi_dst.op == UCC_OP_AVG) return -1;
         for (int j = 0; j < m->n_bufs; j++) { m->dst[j] = a->reduce_multi_dst.dst[j]; m->src1[j] = a->reduce_multi_dst.src1[j]; m->src2[j] = a->reduce_multi_dst.src2[j]; m->counts[j] = a->reduce_multi_dst.counts[j]; }
         return EC_TASK_REDUCE_MULTI_DST; }
     case UCC_EE_EXECUTOR_TASK_COPY: {
@@ -317,10 +319,11 @@ static ucc_status_t exec_task_post(ucc_ee_executor_t *xe, const ucc_ee_executor_
     t->super.eee = xe; t->super.args = *a; t->super.status = UCC_INPROGRESS; t->super.handle = NULL; t->event = NULL; t->slot = NULL;
     if (x->mode == EXEC_MODE_PERSISTENT) {
         ec_ring_slot_t *slot = &x->ring->slots[x->pidx % x->ring->n_slots];
-        if (slot->state == EC_SLOT_POSTED) { ucc_mpool_put(t); return UCC_ERR_NO_RESOURCE; } /* ring full */
+        if (slot->state != EC_SLOT_FREE) { ucc_mpool_put(t); return UCC_ERR_NO_RESOURCE; } /* ring full: the oldest task is not finalized */
         kind = describe(a, slot);
         if (kind < 0) { ucc_mpool_put(t); return UCC_ERR_NOT_SUPPORTED; }
         slot->kind = (uint32_t)kind;
+        slot->seq = x->pidx; /* the worker that serves task pidx takes this slot only for it, not for a task of another lap */
         ucc_memory_cpu_store_fence();
         slot->state = EC_SLOT_POSTED;
         x->pidx++; t->slot = slot;

@@ -14,15 +14,18 @@ template <> struct EcOp<EC_OP_PROD, cuDoubleComplex> { static __device__ __force
 
 static_assert((int)EC_OP_SUM == (int)NVL_OP_SUM && (int)EC_OP_BXOR == (int)NVL_OP_BXOR, "operator enums must line up");
 
-/* x * alpha: integer accumulators are scaled in double precision and truncated (reference ec_cuda_reduce_ops.h: d[i] * alpha),
- * casting alpha (1/N for AVG) to the integer type first would make it 0 */
-template <typename T> __device__ __forceinline__ T scale(T x, double alpha)
+/* x * alpha (AVG: alpha = 1/N).  Floating types multiply by alpha rounded to the accumulator's precision, as ec/cpu and tl/nvl do.
+ * Integer types divide exactly by n = avg_n when alpha is 1/n - the 128-bit ones with tl/nvl's avg_scale / div128_by_small, the
+ * others in their promoted type, since n may exceed the range of an 8- or 16-bit type - and scale in double and truncate for any
+ * other alpha (casting alpha to the integer type would make it 0) */
+template <typename T> __device__ __forceinline__ T scale(T x, double alpha, int n)
 {
-    if constexpr (IsIntAcc<T>::v) return (T)((double)x * alpha);
+    if constexpr (IsInt128<T>::v) return n > 0 ? avg_scale<NVL_OP_AVG, T>(x, 1.0f, n) : (T)((double)x * alpha);
+    else if constexpr (IsIntAcc<T>::v) return n > 0 ? (T)(x / (decltype(x + 0))n) : (T)((double)x * alpha);
     else return (T)(x * (T)alpha);
 }
-template <> __device__ __forceinline__ cuFloatComplex scale(cuFloatComplex x, double a) { return make_cuFloatComplex(x.x * (float)a, x.y * (float)a); }
-template <> __device__ __forceinline__ cuDoubleComplex scale(cuDoubleComplex x, double a) { return make_cuDoubleComplex(x.x * a, x.y * a); }
+template <> __device__ __forceinline__ cuFloatComplex scale(cuFloatComplex x, double a, int) { return make_cuFloatComplex(x.x * (float)a, x.y * (float)a); }
+template <> __device__ __forceinline__ cuDoubleComplex scale(cuDoubleComplex x, double a, int) { return make_cuDoubleComplex(x.x * a, x.y * a); }
 
 static __device__ __forceinline__ const void *src_k(const ec_reduce_args_t &a, int k)
 { return (!a.strided || k == 0) ? a.srcs[a.strided ? 0 : k] : (const char *)a.src2 + (size_t)(k - 1) * a.stride; }
@@ -34,7 +37,7 @@ static __device__ __forceinline__ void reduce_scalar(const ec_reduce_args_t &a, 
     for (size_t i = begin + tid; i < end; i += nt) {
         A acc = ld(ld_elem((const T *)src_k(a, 0) + i));
         for (int k = 1; k < a.n_srcs; k++) acc = EcOp<OP, A>::f(acc, ld(ld_elem((const T *)src_k(a, k) + i)));
-        if (a.with_alpha) acc = scale<A>(acc, a.alpha);
+        if (a.with_alpha) acc = scale<A>(acc, a.alpha, a.avg_n);
         st_elem((T *)a.dst + i, st(acc));
     }
 }
@@ -54,7 +57,7 @@ template <typename T, int OP> static __device__ __forceinline__ void reduce_body
         for (int k = 1; k < a.n_srcs; k++) acc.add(ld_src_v4((const char *)src_k(a, k) + v * 16));
         if (a.with_alpha) {
 #pragma unroll
-            for (int i = 0; i < E; i++) acc.a[i] = scale<A>(acc.a[i], a.alpha);
+            for (int i = 0; i < E; i++) acc.a[i] = scale<A>(acc.a[i], a.alpha, a.avg_n);
         }
         st_v4((char *)a.dst + v * 16, acc.get(1.0f, 1));
     }
@@ -103,7 +106,7 @@ __global__ void __launch_bounds__(1024) ec_reduce_multi_dst_kernel(ec_reduce_mul
     int j = blockIdx.y;
     if (j >= m.n_bufs) return;
     ec_reduce_args_t a; a.dst = m.dst[j]; a.srcs[0] = m.src1[j]; a.srcs[1] = m.src2[j]; a.n_srcs = 2; a.strided = 0; a.src2 = nullptr; a.stride = 0;
-    a.count = m.counts[j]; a.dt = m.dt; a.op = m.op; a.with_alpha = 0; a.alpha = 1.0;
+    a.count = m.counts[j]; a.dt = m.dt; a.op = m.op; a.with_alpha = 0; a.avg_n = 0; a.alpha = 1.0;
     reduce_any(a, EC_GRID_TID, EC_GRID_NT);
 }
 
@@ -128,8 +131,10 @@ __global__ void __launch_bounds__(1024) ec_copy_multi_kernel(ec_copy_multi_args_
 /* ------------------------------------------------------------------ */
 /* persistent executor: worker blocks pop tasks from a host-pinned ring */
 /* (reference ec/cuda/kernel/ec_cuda_executor.cu:125-188: num_workers blocks share one task ring).  Worker block w serves  */
-/* slots w, w + W, w + 2W, ... - the host fills the ring in order, so consecutive tasks land on different workers and     */
-/* run concurrently; inside a task only the worker's own threads take part (tid = threadIdx.x, nt = blockDim.x).        */
+/* tasks w, w + W, w + 2W, ... (task idx in slot idx % n_slots) - the host fills the ring in order, so consecutive tasks  */
+/* land on different workers and run concurrently; inside a task only the worker's own threads take part (tid =         */
+/* threadIdx.x, nt = blockDim.x).  A worker takes a slot only when it holds task idx (slot->seq): when W does not divide  */
+/* n_slots, or exceeds it, the slot may still hold the task of an earlier lap that another worker is running.            */
 /* ------------------------------------------------------------------ */
 __global__ void __launch_bounds__(1024) ec_persistent_kernel(ec_ring_t *ring)
 {
@@ -144,7 +149,10 @@ __global__ void __launch_bounds__(1024) ec_persistent_kernel(ec_ring_t *ring)
             uint32_t cmd;
             for (;;) {
                 if (ring->shutdown) { cmd = 1; break; }
-                if (slot->state == EC_SLOT_POSTED) { cmd = 0; break; }
+                if (slot->state == EC_SLOT_POSTED) {
+                    __threadfence_system(); /* seq is written before the state flip: read it after the state */
+                    if (slot->seq == idx) { cmd = 0; break; }
+                }
             }
             __threadfence_system(); /* arguments written by the host before the state flip are visible now */
             s_cmd = cmd;
@@ -160,7 +168,7 @@ __global__ void __launch_bounds__(1024) ec_persistent_kernel(ec_ring_t *ring)
             ec_reduce_multi_dst_args_t m = slot->u.rmd;
             for (int j = 0; j < m.n_bufs; j++) {
                 ec_reduce_args_t a; a.dst = m.dst[j]; a.srcs[0] = m.src1[j]; a.srcs[1] = m.src2[j]; a.n_srcs = 2; a.strided = 0; a.src2 = nullptr; a.stride = 0;
-                a.count = m.counts[j]; a.dt = m.dt; a.op = m.op; a.with_alpha = 0; a.alpha = 1.0;
+                a.count = m.counts[j]; a.dt = m.dt; a.op = m.op; a.with_alpha = 0; a.avg_n = 0; a.alpha = 1.0;
                 reduce_any(a, tid, nt);
             }
             break; }

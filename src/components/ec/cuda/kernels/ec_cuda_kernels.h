@@ -22,6 +22,7 @@ typedef struct ec_reduce_args {
     int         strided, n_srcs;
     size_t      count;
     int         dt, op, with_alpha;
+    int         avg_n;               /* alpha == 1.0 / avg_n exactly (AVG): integer types divide by it; 0: scale by alpha */
     double      alpha;
 } ec_reduce_args_t;
 typedef struct ec_reduce_multi_dst_args {
@@ -34,6 +35,8 @@ typedef enum { EC_SLOT_FREE = 0, EC_SLOT_POSTED = 1, EC_SLOT_DONE = 2 } ec_slot_
 typedef struct ec_ring_slot {
     volatile uint32_t state;
     uint32_t          kind;
+    volatile uint32_t seq;           /* global index of the task in the slot, written before state becomes POSTED */
+    uint32_t          pad;
     union { ec_reduce_args_t reduce; ec_reduce_multi_dst_args_t rmd; ec_copy_multi_args_t copy; } u;
 } ec_ring_slot_t;
 typedef struct ec_ring { volatile uint32_t shutdown; volatile uint32_t started; uint32_t n_slots; uint32_t pad; ec_ring_slot_t slots[1]; } ec_ring_t;

@@ -1,5 +1,5 @@
 """INT128 / UINT128 on ec/cuda: REDUCE, REDUCE_STRIDED and REDUCE_MULTI_DST for every operator, bitwise against ec/cpu on the same
-inputs (AVG with alpha included: both scale in double and truncate), and an allreduce of CUDA buffers on the host transport
+inputs (AVG with alpha = 1/N included: both divide the wrapped sum by N and truncate), and an allreduce of CUDA buffers on the host transport
 (tl/shm), which reduces through ec/cuda."""
 import numpy as np
 import pytest
