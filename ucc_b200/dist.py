@@ -21,9 +21,20 @@ for _n, _t in (("uint16", "uint16"), ("uint32", "uint32"), ("uint64", "uint64"))
     if hasattr(torch, _n):
         _TORCH_DT[getattr(torch, _n)] = _t
 
+# torch dtypes the library has no datatype for travel as the unsigned integer of their element size, so every data-movement
+# collective moves their bytes unchanged; counts and displacements stay in elements of the tensor
+_CARRIERS = {torch.complex32: "uint32"}
+for _n in ("float8_e4m3fn", "float8_e5m2", "float8_e4m3fnuz", "float8_e5m2fnuz", "float8_e8m0fnu"):
+    if hasattr(torch, _n):
+        _CARRIERS[getattr(torch, _n)] = "uint8"
+_TORCH_DT.update(_CARRIERS)
+
 # a torch.bool tensor goes to the library as uint8 holding 0 / 1: sum is logical or (max), product logical and (min), as in
 # ProcessGroupNCCL; the bitwise and logical operators keep 0 / 1 as they are
 _BOOL_OP = {"sum": "max", "prod": "min"}
+
+# the collectives whose operator the library applies
+REDUCTIONS = frozenset(("allreduce", "reduce", "reduce_scatter", "reduce_scatterv"))
 
 
 def dt_of(t):
@@ -31,12 +42,22 @@ def dt_of(t):
 
 
 def op_of(op, t):
-    """the library operator that computes `op` on the elements of `t`"""
-    if t.dtype != torch.bool:
-        return op
-    if op == "avg":
-        raise ValueError("AVG reduction is not defined for torch.bool tensors")
-    return _BOOL_OP.get(op, op)
+    """(library datatype, library operator, library elements per element of `t`) of the reduction `op` on `t`.
+
+    A complex32 element is two interleaved float16 halves, so its SUM and AVG are the float16 SUM and AVG of twice as many
+    elements.  Every other reduction of a carried dtype (float8, complex32) raises ValueError: the library has no arithmetic for
+    them.  The dtype alone decides, and every member of a collective passes the same dtype, so all of them refuse before
+    any request exists."""
+    if t.dtype == torch.bool:
+        if op == "avg":
+            raise ValueError("AVG reduction is not defined for torch.bool tensors")
+        return "uint8", _BOOL_OP.get(op, op), 1
+    if t.dtype == torch.complex32 and op in ("sum", "avg"):
+        return "float16", op, 2
+    if t.dtype in _CARRIERS:
+        raise ValueError(f"{op.upper()} reduction is not supported for {t.dtype} tensors: the library moves them as "
+                         f"{_CARRIERS[t.dtype]} without arithmetic (complex32 has SUM and AVG, float8 no reduction)")
+    return dt_of(t), op, 1
 
 
 def mem_type_of(t):
@@ -443,9 +464,13 @@ class Communicator:
         ref = dst if dst is not None else src
         if ref is None:  # barrier / fanin / fanout
             return coll_args(coll, root=root, persistent=persistent)
-        return coll_args(coll, dt=dt_of(ref), op=op_of(op, ref), root=root, inplace=inplace, persistent=persistent,
+        dt, op, width = op_of(op, ref) if coll in REDUCTIONS else (dt_of(ref), op, 1)
+        if width != 1:   # counts and displacements in library elements
+            kw = {k: [c * width for c in v] if k in ("src_counts", "src_displs", "dst_counts", "dst_displs") and v is not None else v
+                  for k, v in kw.items()}
+        return coll_args(coll, dt=dt, op=op, root=root, inplace=inplace, persistent=persistent,
                          src_ptr=src.data_ptr() if src is not None else None, dst_ptr=dst.data_ptr() if dst is not None else None,
-                         count_src=src.numel() if src is not None else 0, count_dst=dst.numel() if dst is not None else 0,
+                         count_src=src.numel() * width if src is not None else 0, count_dst=dst.numel() * width if dst is not None else 0,
                          mem_type=mem_type_of(ref), **kw)
 
     def register(self, tensor):

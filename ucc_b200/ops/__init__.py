@@ -3,12 +3,13 @@
 The call shapes follow torch.distributed so a user of `torch.distributed` + ProcessGroupUCC (reference consumer:
 pytorch/torch-ucc) can switch by changing the import.  Every function returns a `Work` whose `.wait()` blocks the
 host; with `async_op=False` (default) the wait is done before returning.  CUDA tensors are posted stream-ordered
-(ucc_collective_triggered_post) on the current stream."""
+(ucc_collective_triggered_post) on the current stream.  float8 and complex32 tensors move byte for byte; of their reductions
+only complex32 SUM / AVG exist, the others raise ValueError (ucc_b200.dist.op_of)."""
 from __future__ import annotations
 
 import torch
 
-from ..dist import Communicator
+from ..dist import Communicator, op_of
 
 _default = None
 
@@ -78,6 +79,7 @@ def all_reduce_from_host(host, out, staging=None, op="sum", comm=None, chunks=No
     reduction overlap instead of adding up.  `staging` (CUDA, same shape) receives the local copy; allocated when omitted.
     Every member must call with the same sizes (the chunking is derived from them).  Returns when `out` is complete."""
     comm = comm or default_comm()
+    op_of(op, out)             # a reduction the library cannot do is refused before any copy is queued
     stream = stream or torch.cuda.current_stream()
     n = host.numel()
     nbytes = n * host.element_size()

@@ -21,7 +21,9 @@ _allgather_base), reduce_scatter (+ _tensor_coalesced, _reduce_scatter_base), al
 send, recv, barrier and the coalescing hooks _start_coalescing / _end_coalescing, so also gather_object, scatter_object_list,
 all_gather_coalesced and _coalescing_manager.  The list forms of allgather, reduce_scatter, gather, scatter and alltoall take
 blocks of any size, zero included.  torch.bool tensors travel as uint8: SUM / MAX are logical or, PRODUCT / MIN logical and, AVG
-is refused.
+is refused.  float8 tensors (float8_e4m3fn, float8_e5m2, their fnuz forms, float8_e8m0fnu) travel as uint8 and complex32 as uint32,
+byte for byte, in every data-movement operation; complex32 SUM / AVG reduce its float16 halves, and every other reduction of these
+dtypes raises a ValueError that names the dtype and the operator, on every rank and before anything is posted.
 Not served, each with an error that names it: ReduceOp.PREMUL_SUM (its factor cannot be read from Python and the library has no
 scaled sum; FSDP2 uses it only for a custom gradient divide factor), recv_anysource (on CUDA tensors a send / recv pair matches in
 post order, so a receive must name its source), monitored_barrier and split_group.
@@ -35,7 +37,7 @@ import itertools
 import torch
 import torch.distributed as dist
 
-from .dist import Communicator
+from .dist import Communicator, op_of
 from .ops import _alltoall_init
 
 _OPS = {dist.ReduceOp.SUM: "sum", dist.ReduceOp.PRODUCT: "prod", dist.ReduceOp.MIN: "min", dist.ReduceOp.MAX: "max", dist.ReduceOp.AVG: "avg",
@@ -53,6 +55,15 @@ def _op(o):
     raise ValueError(f"unsupported reduce op {o}")
 
 
+def _reduce_op(opts, tensors):
+    """the operator of a reduction over `tensors`; a (dtype, operator) pair the library cannot reduce raises ValueError here,
+    before any request of the call exists"""
+    op = _op(opts.reduceOp) if opts is not None else "sum"
+    for t in tensors:
+        op_of(op, t)
+    return op
+
+
 def _flat(n, like):
     """1-D buffer of `n` elements of `like`'s dtype and device, never at address 0, even when `n` is 0"""
     return torch.empty(max(n, 1), dtype=like.dtype, device=like.device)[:n]
@@ -64,9 +75,23 @@ def _views(flat, tensors):
     return [flat[o:o + t.numel()].view(t.shape) for o, t in zip(offs, tensors)]
 
 
+_INT_OF_SIZE = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+
+
+def _copy(dsts, srcs):
+    """dsts[i] <- srcs[i] bit for bit, stream-ordered on CUDA.  torch's CUDA _foreach_copy_ converts floating-point elements
+    through float, which rewrites the NaN payloads of float16, bfloat16 and float8, and it has no float8_e8m0fnu kernel: tensors
+    of one dtype are copied as integers of their element size"""
+    def raw(t):
+        size = t.element_size()
+        return t.view(_INT_OF_SIZE[size]) if size in _INT_OF_SIZE else t.unsqueeze(-1).view(torch.int64)
+    pairs = [(raw(d), raw(s)) if d.dtype == s.dtype else (d, s) for d, s in zip(dsts, srcs)]
+    torch._foreach_copy_([d for d, _ in pairs], [s for _, s in pairs])
+
+
 def _pack(tensors):
     flat = _flat(sum(t.numel() for t in tensors), tensors[0])
-    torch._foreach_copy_(_views(flat, tensors), list(tensors))
+    _copy(_views(flat, tensors), list(tensors))
     return flat
 
 
@@ -179,7 +204,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         posted = None
         if cuda:
             if outs:
-                torch._foreach_copy_(outs, views)
+                _copy(outs, views)
             if wait_posted:   # every kernel is in the stream, a deferred zero-copy launch included: mark the stream behind them
                 stream = torch.cuda.current_stream()
                 posted = (stream, stream.record_event())
@@ -187,7 +212,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         w = _Work(self, reqs, result, cuda, posted=posted)
         if outs and not cuda:
             w.wait()
-            torch._foreach_copy_(outs, views)
+            _copy(outs, views)
         return w
 
     def _reap(self):
@@ -207,7 +232,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     # ---- collectives (list-of-tensors signatures of c10d)
     def allreduce(self, tensors, opts=None):
-        op = _op(opts.reduceOp) if opts is not None else "sum"
+        op = _reduce_op(opts, tensors)
         reqs = [self._comm.allreduce_init(t, t, op=op) for t in tensors]
         return self._run(reqs, tensors, tensors)
 
@@ -221,7 +246,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     def reduce(self, tensors, opts=None):
         root = opts.rootRank if opts is not None else 0
-        op = _op(opts.reduceOp) if opts is not None else "sum"
+        op = _reduce_op(opts, tensors)
         me = self.rank()
         reqs = [self._comm.coll_init("reduce", None if me == root else t, t if me == root else None, op=op, root=root, inplace=me == root) for t in tensors]
         return self._run(reqs, tensors, tensors)
@@ -256,15 +281,15 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         return self._run([self._comm.coll_init("allgather", i.contiguous(), o) for o, i in zip(outputs, inputs)], inputs, outputs)
 
     def _reduce_scatter_base(self, output, input, opts=None):
-        op = _op(opts.reduceOp) if opts is not None else "sum"
+        op = _reduce_op(opts, [input])
         return self._run([self._comm.coll_init("reduce_scatter", input.contiguous(), output, op=op)], [input], output)
 
     def reduce_scatter_tensor_coalesced(self, outputs, inputs, opts=None):
-        op = _op(opts.reduceOp) if opts is not None else "sum"
+        op = _reduce_op(opts, inputs)
         return self._run([self._comm.coll_init("reduce_scatter", i.contiguous(), o, op=op) for o, i in zip(outputs, inputs)], inputs, outputs)
 
     def reduce_scatter(self, outputs, input_lists, opts=None):
-        op = _op(opts.reduceOp) if opts is not None else "sum"
+        op = _reduce_op(opts, outputs)
         reqs, keep = [], []
         for out, ins in zip(outputs, input_lists):
             counts = [t.numel() for t in ins]
