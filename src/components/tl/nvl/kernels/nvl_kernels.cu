@@ -222,6 +222,12 @@ static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int 
     k<<<nblocks, nthreads, 0, s>>>(a);
     return cudaGetLastError();
 }
+/* loads the kernel's module now, where lazy loading would load it at its first launch */
+static cudaError_t nvl_red_load(nvl_red_kernel_t k)
+{
+    struct cudaFuncAttributes fa;
+    return cudaFuncGetAttributes(&fa, reinterpret_cast<const void *>(k));
+}
 extern "C" cudaError_t nvl_launch_exchange(const nvl_xchg_args_t *a, int nblocks, int nthreads, cudaStream_t s)
 {
     if (nthreads > NVL_THREADS_MAX) nthreads = NVL_THREADS_MAX;
@@ -252,6 +258,7 @@ extern "C" cudaError_t nvl_launch_ctrl_init(void *heap_base, cudaStream_t s)
  * run on its emulated stream, which refuses a kernel whose tables reach into a closed IPC mapping */
 extern const nvl_dt_row *const nvl_rows[NVL_DT_LAST];
 static cudaError_t nvl_red_run(nvl_red_kernel_t k, const nvl_red_args_t &a, int nblocks, int nthreads, cudaStream_t s);
+static cudaError_t nvl_red_load(nvl_red_kernel_t) { return cudaSuccess; }
 #endif /* NVL_HOST_EMU */
 
 /* reductions: the datatype predicates and the launchers, the same in the GPU build and in the host-emulated plugin (the entry
@@ -277,6 +284,18 @@ extern "C" cudaError_t nvl_launch_reduce_staged(const nvl_red_args_t *a, int nbl
 { return nvl_red_launch(NVL_FAM_STAGED, a, nblocks, nthreads, s); }
 extern "C" cudaError_t nvl_launch_reduce_direct(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
 { return nvl_red_launch(NVL_FAM_DIRECT, a, nblocks, nthreads, s); }
+extern "C" cudaError_t nvl_launch_reduce_local(const nvl_red_args_t *a, int nthreads, cudaStream_t s)
+{ return nvl_red_launch(NVL_FAM_LOCAL, a, NVL_LOCAL_CTAS, nthreads, s); }
+/* The local kernel follows a barrier kernel that waits for the peers.  Under lazy module loading (the CUDA default) its first
+ * launch would load it while that barrier spins, and when the members are threads of one process the peers' launches queue behind
+ * that load until the barrier gives up: the task loads it at init instead. */
+extern "C" cudaError_t nvl_load_reduce_local(const nvl_red_args_t *ap)
+{
+    const nvl_dt_row *r = nvl_row(ap->dt);
+    nvl_red_args_t a = *ap;
+    const nvl_red_kernel_t k = r ? r->select(NVL_FAM_LOCAL, a) : nullptr;
+    return k ? nvl_red_load(k) : cudaErrorInvalidValue;
+}
 extern "C" cudaError_t nvl_launch_reduce_steps(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s)
 { return nvl_red_launch(NVL_FAM_STEPS, a, nblocks, nthreads, s); }
 #endif

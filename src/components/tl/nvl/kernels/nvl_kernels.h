@@ -15,6 +15,10 @@
 #define NVL_MAX_PEERS  16
 #define NVL_MAX_BLOCKS 320
 #define NVL_LL_MAX     (1024 * 1024)         /* bytes per rank in the one-shot (latency) region */
+/* grid of the local reduction kernel of the copy-engine path, a constant: the path exists to leave the SMs to the application's
+ * kernels, 8 CTAs are 8 of the 132 SMs of an H100, and reducing one heap round of local HBM data is not what bounds that path - the
+ * copy engines' transfers are */
+#define NVL_LOCAL_CTAS 8
 #define NVL_P2P_MAX_CTAS 16                  /* lanes of a point-to-point channel */
 #define NVL_P2P_SLOTS    4                   /* chunks in flight per channel */
 #define NVL_P2P_CHUNK    (256 * 1024)
@@ -189,6 +193,10 @@ cudaError_t  nvl_launch_reduce_staged(const nvl_red_args_t *a, int nblocks, int 
 cudaError_t  nvl_launch_reduce_scatter_oneshot(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s);
 /* zero-copy two-shot: every rank reduces its slice straight out of the members' src buffers into their dst buffers */
 cudaError_t  nvl_launch_reduce_direct(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s);
+/* local N-source reduction of the copy-engine path: a->d.src[i] = a->count elements of my i-th right neighbour's block (i = 0:
+ * mine), already in local memory, reduced into a->dst, on NVL_LOCAL_CTAS CTAs */
+cudaError_t  nvl_launch_reduce_local(const nvl_red_args_t *a, int nthreads, cudaStream_t s);
+cudaError_t  nvl_load_reduce_local(const nvl_red_args_t *a);   /* its module, loaded ahead of the first launch */
 /* ring / recursive halving-doubling allreduce and reduce_scatter(v) through the heaps (a->sched), single round */
 cudaError_t  nvl_launch_reduce_steps(const nvl_red_args_t *a, int nblocks, int nthreads, cudaStream_t s);
 /* staged NVLS allreduce with three heap buffers: staging / in-switch reduction / copy-out of consecutive chunks overlap */

@@ -414,6 +414,39 @@ template <typename T, int OP, int CN> __global__ void __launch_bounds__(NVL_BW_T
 }
 
 /* ------------------------------------------------------------------ */
+/* local N-source reduction (the copy-engine reduction path)           */
+/*   The copy engines have already brought the peers' blocks into my   */
+/*   heap; this kernel reduces N LOCAL sources into one destination:   */
+/*   no barrier, no flag, no peer access.                              */
+/* ------------------------------------------------------------------ */
+/* a.d.src[i] = the block of my i-th right neighbour (i = 0: my own), a.count elements each, result -> a.dst.  The sources come in
+ * the rotated order of the zero-copy two-shot kernel and go through the same reduce_core, operator bodies, accumulators and AVG
+ * scaling, so a copy-engine reduction gives the bits of twoshot_zcopy(direct) for the same inputs.
+ * Grid: NVL_LOCAL_CTAS CTAs (nvl_kernels.h), whatever the size. */
+template <typename T, int OP, int CN> __global__ void __launch_bounds__(NVL_BW_THREADS, 2) nvl_reduce_local_kernel_t(const __grid_constant__ nvl_red_args_t a)
+{
+    constexpr int E = 16 / sizeof(T);
+    typedef typename AccOf<T>::type A;
+    const int N = CN ? CN : a.team.size, nb = gridDim.x, b = blockIdx.x;
+    const size_t cnt = a.count, nfull = cnt / E, per = (nfull + nb - 1) / nb;
+    const size_t j0 = dmin((size_t)b * per, nfull), j1 = dmin(j0 + per, nfull);
+    const float inv_n = 1.0f / (float)N;
+    T *const dst = static_cast<T *>(a.dst);
+    const bool dal = ((uintptr_t)dst & 15) == 0;
+    auto src_of = [&](int i) -> const char * { return a.d.src[i]; };
+    auto store = [&](size_t jj, uint4 r) { store_dst_vec<T>(dst, jj * E, cnt, dal, r); };
+    reduce_core<T, OP, CN, RedShape<CN>::NP, RedShape<CN>::U>(N, j0, j1, inv_n, src_of, store);
+    /* ragged tail (fewer than E elements): as in direct_body */
+    if (b == nb - 1 && threadIdx.x == 0 && nfull * E < cnt) {
+        for (size_t e = nfull * E; e < cnt; e++) {
+            A acc = to_acc<T>(reinterpret_cast<const T *>(a.d.src[0])[e]);
+            for (int i = 1; i < N; i++) acc = OpFn<OP, A>::f(acc, to_acc<T>(reinterpret_cast<const T *>(a.d.src[i])[e]));
+            dst[e] = from_acc<T>(avg_scale<OP, A>(acc, inv_n, N));
+        }
+    }
+}
+
+/* ------------------------------------------------------------------ */
 /* step-structured allreduce / reduce_scatter through the heaps:       */
 /*   sched 1: ring (N-1 reduce-scatter steps + N-1 allgather steps,    */
 /*            neighbour links only)                                    */
@@ -558,7 +591,7 @@ template <typename T, int OP> __global__ void __launch_bounds__(NVL_BW_THREADS, 
 /* a __global__ function on the GPU (launched with <<<>>>); in the host emulation the same function compiled as C++, called by
  * every emulated thread */
 typedef void (*nvl_red_kernel_t)(nvl_red_args_t);
-enum { NVL_FAM_ONESHOT, NVL_FAM_ONESHOT_RS, NVL_FAM_STAGED, NVL_FAM_DIRECT, NVL_FAM_STEPS, NVL_FAM_PIPE, NVL_FAM_SYMM };
+enum { NVL_FAM_ONESHOT, NVL_FAM_ONESHOT_RS, NVL_FAM_STAGED, NVL_FAM_DIRECT, NVL_FAM_STEPS, NVL_FAM_PIPE, NVL_FAM_SYMM, NVL_FAM_LOCAL };
 
 /* the kernel of family fam for (T, OP) and the team-size class / NVLS mode of a; null when there is none (the NVLS kernels exist
  * for the pairs the switch can reduce only).  The zero-copy kernel gets a's pointer tables rotated (nvl_direct_rotate). */
@@ -585,6 +618,13 @@ template <typename T, int OP> static nvl_red_kernel_t nvl_select_op(int fam, nvl
         case 8: return nvl_reduce_direct_kernel_t<T, OP, 8>;
         default: return nvl_reduce_direct_kernel_t<T, OP, 0>;
         }
+    case NVL_FAM_LOCAL: /* the host builds its tables rotated */
+        switch (nvl_size_class(a.team.size)) {
+        case 2: return nvl_reduce_local_kernel_t<T, OP, 2>;
+        case 4: return nvl_reduce_local_kernel_t<T, OP, 4>;
+        case 8: return nvl_reduce_local_kernel_t<T, OP, 8>;
+        default: return nvl_reduce_local_kernel_t<T, OP, 0>;
+        }
     case NVL_FAM_PIPE: if constexpr (mc) return nvl_allreduce_nvls_pipe_kernel_t<T, OP>; else return nullptr;
     case NVL_FAM_SYMM: if constexpr (mc) return nvl_allreduce_symm_kernel_t<T, OP>; else return nullptr;
     default: return nullptr;
@@ -610,6 +650,7 @@ template <typename T> static void nvl_reduce_direct_kernel(nvl_red_args_t a) { n
 template <typename T> static void nvl_reduce_steps_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_STEPS, a); }
 template <typename T> static void nvl_allreduce_nvls_pipe_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_PIPE, a); }
 template <typename T> static void nvl_allreduce_symm_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_SYMM, a); }
+template <typename T> static void nvl_reduce_local_kernel(nvl_red_args_t a) { nvl_emu_run<T>(NVL_FAM_LOCAL, a); }
 #endif
 
 /* one datatype as the host sees it: nvl_red_<dt>.cu defines the row of its type, nvl_kernels.cu tables the rows by nvl_dt_t */

@@ -188,6 +188,8 @@ typedef enum {
     NVL_PATH_RHD,          /* step-structured reduction, recursive halving / doubling */
     NVL_PATH_NVLS_PIPE,    /* pipelined staged NVLS allreduce (kernels/nvl_pipe.cuh) */
     NVL_PATH_SYMM,         /* NVLS reduction on symmetric user memory, nothing staged (kernels/nvl_symm.cuh) */
+    NVL_PATH_RED_CE,       /* allreduce / reduce_scatter(v) under UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU; direct: the copy engines pull
+                              the peers' blocks into my heap, a small local kernel reduces them; staged: the two-shot staged kernel */
     NVL_PATH_AG_SYMM,      /* allgather into a symmetric destination by multimem.st (u.xchg: src, src_bytes, dst, push_off) */
     NVL_PATH_PULL,         /* stage + pull exchange; direct: pull from the members' source buffers */
     NVL_PATH_PULL_NVLS,    /* exchange whose staging multicasts into every heap (u.xchg.use_mc) */
@@ -195,6 +197,8 @@ typedef enum {
     NVL_PATH_PUSH,         /* direct: store my blocks into the members' destinations (kernels/nvl_push.cu); staged: pull */
     NVL_PATH_PUSH_BULK,    /* the same, moved by TMA bulk copies */
     NVL_PATH_PUSH_CE,      /* the same, one cudaMemcpyAsync per peer between two barrier kernels */
+    NVL_PATH_XCHG_CE,      /* bcast / gather(v) / scatter(v) under the overlap hint; direct: cudaMemcpyAsync to / from the root's mapped
+                              buffer between two barrier kernels; staged: pull */
     NVL_PATH_SWAP,         /* in-place alltoall(v); direct: pairwise swap kernel (kernels/nvl_swap.cu); staged: self-copy + pull */
     NVL_PATH_SELF_COPY,    /* team of one: u.xchg.{dst,src,src_bytes} describe the only data movement, copied by a kernel */
     NVL_PATH_SELF_COPY_CE, /* ... copied by cudaMemcpyAsync */
@@ -243,7 +247,8 @@ typedef struct ucc_tl_nvl_task {
     int                 rz_stream_idle;/* recv: the stream had nothing queued at post time */
     int                 rz_pub_pending;/* recv: the buffer is not on the board yet (stream not there yet / slot busy / not my turn) */
     nvl_xb_buf_t        rz_buf;        /* recv: what will be published */
-    /* push paths: what the direct form stores where */
+    /* push paths: what the direct form stores where (XCHG_CE: recv_off = what the root publishes for member p - where p's block
+     * lands in the root's destination (gather(v)) or starts in its source (scatter(v)); peer_land[root] = that entry for me) */
     struct { size_t send_off[NVL_MAX_PEERS], send_bytes[NVL_MAX_PEERS], land_off[NVL_MAX_PEERS], recv_off[NVL_MAX_PEERS], peer_land[NVL_MAX_PEERS]; int lookup; } push;
 } ucc_tl_nvl_task_t;
 

@@ -35,6 +35,10 @@ static int to_nvl_op(ucc_reduction_op_t op)
  * stores, which are correct for managed pages wherever they live.  A managed buffer is never mapped by a peer (tl_nvl_direct.c:
  * export_buf), so its collectives run the staged forms. */
 static inline int is_cuda(ucc_memory_type_t mt) { return mt == UCC_MEMORY_TYPE_CUDA || mt == UCC_MEMORY_TYPE_CUDA_MANAGED; }
+/* UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU: the caller runs its own kernels next to this collective and prefers an implementation that
+ * leaves the SMs to them.  Every member passes the same flags (a collective argument), so every member takes the same path. */
+static inline int overlap_gpu(const ucc_coll_args_t *a)
+{ return (a->mask & UCC_COLL_ARGS_FIELD_FLAGS) && (a->flags & UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU); }
 
 /* ------------------------------------------------------------------ */
 /* task life cycle                                                     */
@@ -44,8 +48,8 @@ static cudaEvent_t event_get(ucc_tl_nvl_context_t *ctx);
 static char nvl_last_launch[128];
 UCC_EXPORT const char *ucc_tl_nvl_last_launch_info(void) { return nvl_last_launch; }
 /* launch notes of each path's staged and direct form.  threads / grid: what the note reports where that is not the task's nthreads /
- * nblocks (grid -1: no grid) */
-typedef struct { const char *staged, *direct; int direct_threads, grid; } nvl_path_note_t;
+ * nblocks (grid -1: no grid); direct_grid: the same for the direct form alone */
+typedef struct { const char *staged, *direct; int direct_threads, grid, direct_grid; } nvl_path_note_t;
 static const nvl_path_note_t nvl_path_notes[NVL_PATH_NUM] = {
     [NVL_PATH_ONESHOT]      = {"oneshot"},
     [NVL_PATH_ONESHOT_RS]   = {"oneshot_rs"},
@@ -55,13 +59,15 @@ static const nvl_path_note_t nvl_path_notes[NVL_PATH_NUM] = {
     [NVL_PATH_RHD]          = {"rhd"},
     [NVL_PATH_NVLS_PIPE]    = {"nvls_pipe"},
     [NVL_PATH_SYMM]         = {"nvls_symm_inplace"},
+    [NVL_PATH_RED_CE]       = {"twoshot_staged", "reduce_copy_engine", 0, 0, NVL_LOCAL_CTAS},
     [NVL_PATH_AG_SYMM]      = {"allgather_symm_mc"},
     [NVL_PATH_PULL]         = {"exchange_pull_staged", "exchange_pull_zcopy"},
     [NVL_PATH_PULL_NVLS]    = {"exchange_nvls"},
     [NVL_PATH_PULL_RING]    = {"exchange_ring"},
     [NVL_PATH_PUSH]         = {"exchange_pull_staged", "exchange_push"},
     [NVL_PATH_PUSH_BULK]    = {"exchange_pull_staged", "exchange_push_bulk(tma)", 32},
-    [NVL_PATH_PUSH_CE]      = {"exchange_pull_staged", "exchange_push_copy_engine"},
+    [NVL_PATH_PUSH_CE]      = {"exchange_pull_staged", "exchange_push_copy_engine", 0, 0, 1},
+    [NVL_PATH_XCHG_CE]      = {"exchange_pull_staged", "exchange_copy_engine", 32, 0, 1},
     [NVL_PATH_SWAP]         = {"exchange_pull_staged_inplace", "exchange_swap"},
     [NVL_PATH_SELF_COPY]    = {"self_copy"},
     [NVL_PATH_SELF_COPY_CE] = {"self_copy(cudaMemcpyAsync)", NULL, 0, -1},
@@ -69,6 +75,8 @@ static const nvl_path_note_t nvl_path_notes[NVL_PATH_NUM] = {
 };
 static inline int path_uses_xchg(nvl_path_t p) { return p >= NVL_PATH_AG_SYMM && p <= NVL_PATH_SELF_COPY_CE; }
 static inline int path_is_push(nvl_path_t p) { return p == NVL_PATH_PUSH || p == NVL_PATH_PUSH_BULK || p == NVL_PATH_PUSH_CE; }
+/* the members publish an offset table with their buffers (t->push.recv_off) and read theirs back (t->push.peer_land) */
+static inline int path_has_aux(nvl_path_t p) { return path_is_push(p) || p == NVL_PATH_XCHG_CE; }
 /* this post runs the direct form of its path: the members' buffers resolved */
 static inline int task_runs_direct(const ucc_tl_nvl_task_t *t)
 { return path_uses_xchg(t->path) ? t->u.xchg.direct : t->u.red.direct != NVL_DIRECT_NONE; }
@@ -86,8 +94,8 @@ static void note_launch(const ucc_tl_nvl_task_t *t)
     }
     if (n->grid < 0) { snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s", n->staged); return; }
     direct = task_runs_direct(t);
-    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", direct ? n->direct : n->staged, n->grid ? n->grid : t->nblocks,
-             direct && n->direct_threads ? n->direct_threads : t->nthreads);
+    snprintf(nvl_last_launch, sizeof(nvl_last_launch), "%s %dx%d", direct ? n->direct : n->staged,
+             direct && n->direct_grid ? n->direct_grid : (n->grid ? n->grid : t->nblocks), direct && n->direct_threads ? n->direct_threads : t->nthreads);
 }
 
 /* in-place alltoall(v).  Buffers resolved: one swap kernel trades every pair of regions between the mapped buffers.  Otherwise my
@@ -144,6 +152,77 @@ static cudaError_t launch_push(ucc_tl_nvl_task_t *t, cudaStream_t s)
     return e;
 }
 
+/* copy-engine reduction (allreduce / reduce_scatter(v) under the overlap hint), every member's source (and, allreduce, destination)
+ * mapped: barrier kernel (every member's source is final and its destination may be written) -> per round, one DMA per peer of
+ * its part of my slice out of its mapped source into my heap's data region, then the local reduction kernel (NVL_LOCAL_CTAS CTAs)
+ * of the N sources into my destination -> allreduce: one DMA of my reduced slice into every peer's mapped destination -> barrier
+ * kernel.  Rounds reuse the data region in stream order.  In place works: only the slice's owner writes a slice, after it has
+ * pulled it. */
+static cudaError_t launch_red_ce(ucc_tl_nvl_task_t *t, cudaStream_t s)
+{
+    const nvl_red_args_t *r = &t->u.red;
+    const int N = r->team.size, me = r->team.rank;
+    const size_t dts = nvl_dt_size(r->dt), cap = r->team.data_size / (size_t)(N - 1) / 16 * 16 / dts; /* elements per peer and round */
+    char *const data = r->team.heap[me] + NVL_DATA_OFFSET;
+    size_t off, cnt; /* my slice: first element, elements */
+    nvl_red_args_t k;
+    cudaError_t e;
+    if (r->kind == NVL_RED_REDUCE_SCATTER) { off = r->rs_offset[me]; cnt = r->rs_count[me]; }
+    else { /* the slices of the two-shot kernels (make_plan) */
+        const size_t E = 16 / dts, se = ucc_div_round_up(ucc_div_round_up(r->count, (size_t)N), E) * E;
+        off = ucc_min((size_t)me * se, r->count); cnt = ucc_min(se, r->count - off);
+    }
+    memset(&k, 0, sizeof(k));
+    k.team = r->team; k.dt = r->dt; k.op = r->op; k.kind = r->kind;
+    e = nvl_launch_barrier(&r->team, s);
+    for (size_t done = 0; done < cnt && e == cudaSuccess; done += cap) {
+        const size_t c = ucc_min(cap, cnt - done), so = (off + done) * dts;
+        k.count = c;
+        k.d.src[0] = (const char *)r->src + so;
+        for (int i = 1; i < N && e == cudaSuccess; i++) {
+            char *slot = data + (size_t)(i - 1) * cap * dts;
+            k.d.src[i] = slot;
+            e = cudaMemcpyAsync(slot, r->d.src[(me + i) % N] + so, c * dts, cudaMemcpyDeviceToDevice, s);
+        }
+        k.dst = (char *)r->dst + (r->kind == NVL_RED_REDUCE_SCATTER ? done * dts : so);
+        if (e == cudaSuccess) e = nvl_launch_reduce_local(&k, t->nthreads, s);
+    }
+    for (int i = 1; i < N && cnt && e == cudaSuccess && r->kind == NVL_RED_ALLREDUCE; i++)
+        e = cudaMemcpyAsync(r->d.dst[(me + i) % N] + off * dts, (const char *)r->dst + off * dts, cnt * dts, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = nvl_launch_barrier(&r->team, s);
+    return e;
+}
+
+/* copy-engine bcast / gather(v) / scatter(v) under the overlap hint, the root's buffer mapped: barrier kernel -> at most one DMA per
+ * member (a non-root copies the root's source into its buffer, its block into the root's destination or its block out of the
+ * root's source; the root of a gather / scatter that is not in place copies its own block locally) -> barrier kernel.  Where a
+ * block lies in the root's buffer of a gatherv / scatterv only the root knows: it published it (peer_land). */
+static cudaError_t launch_xchg_ce(ucc_tl_nvl_task_t *t, cudaStream_t s)
+{
+    const nvl_xchg_args_t *x = &t->u.xchg;
+    const ucc_coll_args_t *a = &t->super.bargs.args;
+    const int me = x->team.rank, root = (int)a->root;
+    const char *from = NULL; char *to = NULL; size_t len = 0;
+    cudaError_t e;
+    switch (a->coll_type) {
+    case UCC_COLL_TYPE_BCAST:
+        if (me != root) { to = (char *)x->dst; from = x->d.src[root]; len = x->pull_bytes[root]; }
+        break;
+    case UCC_COLL_TYPE_GATHER: case UCC_COLL_TYPE_GATHERV:
+        if (me != root) { to = x->d.dst[root] + t->push.peer_land[root]; from = (const char *)x->src; len = x->src_bytes; }
+        else { to = (char *)x->dst + x->dst_off[me]; from = (const char *)x->src; len = to != from ? x->pull_bytes[me] : 0; }
+        break;
+    default: /* scatter(v) */
+        if (me != root) { to = (char *)x->dst; from = x->d.src[root] + t->push.peer_land[root]; len = x->pull_bytes[root]; }
+        else if (x->dst) { to = (char *)x->dst; from = (const char *)x->src + x->self_off; len = x->pull_bytes[me]; }
+        break;
+    }
+    e = nvl_launch_barrier(&x->team, s);
+    if (e == cudaSuccess && len) e = cudaMemcpyAsync(to, from, len, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = nvl_launch_barrier(&x->team, s);
+    return e;
+}
+
 static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
 {
     const nvl_xchg_args_t *x = &t->u.xchg;
@@ -155,6 +234,9 @@ static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
     case NVL_PATH_TWOSHOT:
         if (task_runs_direct(t)) { e = nvl_launch_reduce_direct(&t->u.red, t->nblocks, t->nthreads, s); break; }
         /* fall through */
+    case NVL_PATH_RED_CE:
+        if (task_runs_direct(t)) { e = launch_red_ce(t, s); break; }
+        /* fall through */
     case NVL_PATH_NVLS: e = nvl_launch_reduce_staged(&t->u.red, t->nblocks, t->nthreads, s); break;
     case NVL_PATH_RING: case NVL_PATH_RHD: e = nvl_launch_reduce_steps(&t->u.red, t->nblocks, t->nthreads, s); break;
     case NVL_PATH_NVLS_PIPE: e = nvl_launch_reduce_pipe(&t->u.red, t->nblocks, t->nthreads, s); break;
@@ -163,6 +245,9 @@ static ucc_status_t nvl_launch(ucc_tl_nvl_task_t *t, cudaStream_t s)
     case NVL_PATH_PUSH: case NVL_PATH_PUSH_BULK: case NVL_PATH_PUSH_CE:
         /* (every member takes the direct form or none: `direct` is decided from what all of them published) */
         if (task_runs_direct(t)) { e = launch_push(t, s); break; }
+        /* fall through */
+    case NVL_PATH_XCHG_CE:
+        if (t->path == NVL_PATH_XCHG_CE && task_runs_direct(t)) { e = launch_xchg_ce(t, s); break; }
         /* fall through */
     case NVL_PATH_PULL: case NVL_PATH_PULL_NVLS: case NVL_PATH_PULL_RING: e = nvl_launch_exchange(x, t->nblocks, t->nthreads, s); break;
     case NVL_PATH_SWAP: e = launch_swap(t, s); break;
@@ -207,7 +292,7 @@ static void task_set_lane(ucc_tl_nvl_task_t *t, unsigned lane)
  * members' buffers are not all known yet) */
 static ucc_status_t task_set_direct(ucc_tl_nvl_task_t *t)
 {
-    int push = path_is_push(t->path), direct;
+    int push = path_has_aux(t->path), direct;
     ucc_status_t st;
     if (!t->zc.flags) return UCC_OK;
     st = ucc_tl_nvl_zc_ready(t->team, &t->zc, UCC_IS_PERSISTENT(t->super.bargs.args), push ? t->push.recv_off : NULL, push ? t->push.peer_land : NULL, &direct);
@@ -465,7 +550,7 @@ static ucc_status_t nvl_post_on(ucc_tl_nvl_task_t *t, cudaStream_t s)
         return ucc_progress_queue_enqueue(UCC_TL_CORE_CTX(t->team)->pq, &t->super);
     }
     if (t->path != NVL_PATH_SELF_COPY && t->path != NVL_PATH_SELF_COPY_CE) task_set_lane(t, team->lane_seq++ % team->nlanes);
-    if (t->zc.flags) ucc_tl_nvl_zc_post(team, &t->zc, t->captured, path_is_push(t->path) ? t->push.recv_off : NULL);
+    if (t->zc.flags) ucc_tl_nvl_zc_post(team, &t->zc, t->captured, path_has_aux(t->path) ? t->push.recv_off : NULL);
     /* a captured post never waits: it has cached tables or runs staged */
     st = t->captured || ucc_list_is_empty(&team->launch_q) ? task_set_direct(t) : UCC_INPROGRESS;
     if (st == UCC_OK) st = launch_ordered(t, s);
@@ -610,8 +695,9 @@ static ucc_status_t self_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
      * TMA ring; 64 MB 47.7 us against 49.7 us for the thread copy below; 16 MB 8.9 us against 11.1 us.  Smaller copies, not
      * measured against it, keep the thread copy.  A managed side always takes the thread copy, as a precaution (cudaMemcpyAsync on
      * managed pages was not measured): the kernel's loads and stores are correct for its pages wherever they live, where
-     * cudaMemcpyAsync would be handed a device-to-device kind for them. */
-    st = task_alloc(b, b_team, copy >= ((size_t)16 << 20) && smt == UCC_MEMORY_TYPE_CUDA && dmt == UCC_MEMORY_TYPE_CUDA ? NVL_PATH_SELF_COPY_CE : NVL_PATH_SELF_COPY, &t);
+     * cudaMemcpyAsync would be handed a device-to-device kind for them.  Under the overlap hint device buffers take cudaMemcpyAsync
+     * at every size: it occupies no SM. */
+    st = task_alloc(b, b_team, (copy >= ((size_t)16 << 20) || (copy && overlap_gpu(a))) && smt == UCC_MEMORY_TYPE_CUDA && dmt == UCC_MEMORY_TYPE_CUDA ? NVL_PATH_SELF_COPY_CE : NVL_PATH_SELF_COPY, &t);
     if (st != UCC_OK) return st;
     memset(&t->u.xchg, 0, sizeof(t->u.xchg));
     t->u.xchg.src = src; t->u.xchg.dst = dst; t->u.xchg.src_bytes = copy;
@@ -647,6 +733,8 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
     ucc_coll_args_t *a = &b->args;
     ucc_rank_t N = UCC_TL_TEAM_SIZE(team), me = UCC_TL_TEAM_RANK(team);
     int inplace = UCC_IS_INPLACE(*a), root = (ucc_rank_t)a->root == me;
+    /* under the overlap hint every algorithm of allreduce / reduce_scatter(v) maps to the copy-engine path (reduce has no such form) */
+    int ce = overlap_gpu(a) && a->coll_type != UCC_COLL_TYPE_REDUCE;
     ucc_tl_nvl_task_t *t;
     nvl_red_args_t r;
     nvl_path_t path;
@@ -677,6 +765,11 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
     ndt = to_nvl_dt(dt); nop = to_nvl_op(a->op);
     if (ndt < 0 || nop < 0 || !nvl_dt_supports_op(ndt, nop)) return UCC_ERR_NOT_SUPPORTED;
     bytes = count * ucc_dt_size(dt);
+    if (ce) {
+        alg = RED_ALG_TWOSHOT;
+        /* the direct form gives every peer a part of the data region per round, the staged one every member */
+        if (ctx->cfg.symmetric_size / N < 16) return UCC_ERR_NOT_SUPPORTED;
+    }
     if (alg == RED_ALG_ONESHOT) {
         /* allreduce: the whole vector goes into a 1 MB slot; reduce_scatter(v): every block does (kernels/nvl_oneshot_rs.cuh) */
         size_t need = bytes;
@@ -740,10 +833,16 @@ static ucc_status_t red_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, u
      * knows (can the buffer be exported? is it aligned?) travels with the exchange.  The NVLS kernels stay staged: writing the
      * result to N mapped destinations (NVL_DIRECT_DST) instead of one multicast store multiplies the bytes leaving each GPU by
      * 1.75 on 8 members.  Reduce_scatter maps the sources only, reduce uses no registrations. */
+    if (ce && path == NVL_PATH_TWOSHOT) {
+        path = NVL_PATH_RED_CE; /* (the symmetric user region keeps its in-switch path) */
+        if (nvl_load_reduce_local(&r) != cudaSuccess) { (void)cudaGetLastError(); return UCC_ERR_NOT_SUPPORTED; }
+    }
     st = task_alloc(b, b_team, path, &t);
     if (st != UCC_OK) return st;
     t->u.red = r; t->nblocks = nb;
-    if (path == NVL_PATH_TWOSHOT && ctx->cfg.zcopy != UCC_NO && bytes >= ctx->cfg.zcopy_thresh && (r.kind != NVL_RED_REDUCE_SCATTER || rs_offsets_aligned(&r, dt))) {
+    /* the copy-engine path maps the same buffers as the zero-copy two-shot kernel, at every size */
+    if (((path == NVL_PATH_TWOSHOT && bytes >= ctx->cfg.zcopy_thresh) || path == NVL_PATH_RED_CE) && ctx->cfg.zcopy != UCC_NO &&
+        (r.kind != NVL_RED_REDUCE_SCATTER || rs_offsets_aligned(&r, dt))) {
         int rs = r.kind == NVL_RED_REDUCE_SCATTER;
         ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_SRC | NVL_ZC_ALIGN | (rs ? 0 : NVL_ZC_DST), src, bytes, rs ? NULL : dst, bytes, r.kind != NVL_RED_REDUCE ? a : NULL);
     }
@@ -856,6 +955,9 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     ucc_coll_type_t ct = a->coll_type;
     int inplace = UCC_IS_INPLACE(*a), a2a = ct == UCC_COLL_TYPE_ALLTOALL || ct == UCC_COLL_TYPE_ALLTOALLV;
     int ag = ct == UCC_COLL_TYPE_ALLGATHER || ct == UCC_COLL_TYPE_ALLGATHERV;
+    /* under the overlap hint every algorithm maps to a copy-engine path: allgather(v) / alltoall(v) to the copy-engine push, bcast /
+     * gather(v) / scatter(v) to the copy-engine exchange; in-place alltoall(v) stays on swap, send / recv on its channel */
+    int ce = overlap_gpu(a) && !UCC_COLL_ARGS_ACTIVE_SET(a) && !team->self;
     /* alltoallv / gatherv / scatterv: `moved` is private to a rank, so no decision may depend on it */
     int private_sizes = ct == UCC_COLL_TYPE_ALLTOALLV || ct == UCC_COLL_TYPE_GATHERV || ct == UCC_COLL_TYPE_SCATTERV;
     size_t cap = ctx->cfg.symmetric_size > NVL_XCHG_TABLE_BYTES ? ctx->cfg.symmetric_size - NVL_XCHG_TABLE_BYTES : 0;
@@ -864,7 +966,11 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
     ucc_tl_nvl_task_t *t;
     int nb;
     ucc_status_t st;
-    if (path_is_push(path) && ((!ag && !a2a) || (!team->self && (!team->zcopy || ctx->cfg.zcopy == UCC_NO)))) return UCC_ERR_NOT_SUPPORTED;
+    if (ce && (ag || a2a) && !(a2a && inplace)) path = NVL_PATH_PUSH_CE;
+    else if (ce && !ag && !a2a) path = NVL_PATH_XCHG_CE;
+    else if (ce && path_is_push(path)) path = NVL_PATH_PULL; /* in-place alltoall(v) -> swap below */
+    /* (the copy-engine paths of the hint run their staged form where zero-copy is off) */
+    if (path_is_push(path) && ((!ag && !a2a) || (!ce && !team->self && (!team->zcopy || ctx->cfg.zcopy == UCC_NO)))) return UCC_ERR_NOT_SUPPORTED;
     if (path_is_push(path) && a2a && inplace) return UCC_ERR_NOT_SUPPORTED; /* -> swap, through the score fallback */
     if (path == NVL_PATH_PULL_NVLS && (!team->nvls || (!ag && ct != UCC_COLL_TYPE_BCAST))) return UCC_ERR_NOT_SUPPORTED;
     if (path == NVL_PATH_PULL_RING && !ag) return UCC_ERR_NOT_SUPPORTED;
@@ -932,7 +1038,7 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
                 path = NVL_PATH_PUSH_BULK; nb = (int)ucc_max(1u, ucc_min(ctx->cfg.bulk_ctas, ctx->cfg.max_blocks));
             }
         }
-        if (path == NVL_PATH_PUSH_CE) nb = 1;
+        if (path == NVL_PATH_PUSH_CE && !ce) nb = 1; /* (its staged form is then the pull kernel on one CTA) */
     }
     st = task_alloc(b, b_team, path, &t);
     if (st != UCC_OK) return st;
@@ -963,11 +1069,27 @@ static ucc_status_t xchg_init(ucc_base_coll_args_t *b, ucc_base_team_t *b_team, 
             else { t->push.send_off[p] = 0; t->push.send_bytes[p] = x.pull_bytes[me]; t->push.land_off[p] = x.dst_off[me]; } /* my block, at my displacement, in everybody's dst */
             if (x.dst_off[p] + x.pull_bytes[p] > dst_len) dst_len = x.dst_off[p] + x.pull_bytes[p];
         }
-        ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, x.dst, dst_len, NULL);
+        if (ctx->cfg.zcopy != UCC_NO) ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, x.dst, dst_len, NULL);
         /* the direct forms of bulk and ce hand my source to the TMA engine or the copy engines.  As a precaution (not measured on
          * managed pages) a managed source withdraws my destination there, and every member runs the staged pull; the thread push
          * reads my source with ordinary loads and keeps its direct form */
         if (t->zc.flags && (path == NVL_PATH_PUSH_BULK || path == NVL_PATH_PUSH_CE) && ucc_tl_nvl_is_managed(x.src)) t->zc.flags |= NVL_ZC_WITHDRAW;
+    }
+    if (path == NVL_PATH_XCHG_CE && ctx->cfg.zcopy != UCC_NO) {
+        /* the root's buffer travels over the exchange board: its source (bcast, scatter(v)) or destination (gather(v)).  The root
+         * publishes where each member's block starts in it; bcast buffers may also come from registrations, which every member
+         * holds.  As with the copy-engine push, a managed buffer of mine withdraws, and every member runs the staged pull. */
+        const int is_root = (ucc_rank_t)a->root == me;
+        memset(t->push.recv_off, 0, sizeof(t->push.recv_off));
+        if (ct == UCC_COLL_TYPE_BCAST) ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_SRC, x.src, is_root ? x.src_bytes : x.pull_bytes[a->root], NULL, 0, a);
+        else if (ct == UCC_COLL_TYPE_GATHER || ct == UCC_COLL_TYPE_GATHERV) {
+            for (ucc_rank_t p = 0; p < N && is_root; p++) { t->push.recv_off[p] = x.dst_off[p]; dst_len = ucc_max(dst_len, x.dst_off[p] + x.pull_bytes[p]); }
+            ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_DST, NULL, 0, is_root ? x.dst : NULL, dst_len, NULL);
+        } else {
+            for (ucc_rank_t p = 0; p < N && is_root; p++) t->push.recv_off[p] = ct == UCC_COLL_TYPE_SCATTERV ? x.stage_off[p] : p * (x.src_bytes / N);
+            ucc_tl_nvl_zc_init(team, &t->zc, NVL_ZC_SRC, is_root ? x.src : NULL, is_root ? x.src_bytes : 0, NULL, 0, NULL);
+        }
+        if (t->zc.flags && (ucc_tl_nvl_is_managed(x.src) || ucc_tl_nvl_is_managed(x.dst))) t->zc.flags |= NVL_ZC_WITHDRAW;
     }
     *task_p = &t->super;
     return UCC_OK;

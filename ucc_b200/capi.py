@@ -82,6 +82,9 @@ UCC_EP_MAP_FULL, UCC_EP_MAP_STRIDED, UCC_EP_MAP_ARRAY, UCC_EP_MAP_CB = 1, 2, 3, 
  UCC_COLL_ARGS_FIELD_ACTIVE_SET) = [BIT(i) for i in range(5)]
 UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH, UCC_COLL_ARGS_FIELD_MEM_MAP_DST_MEMH = BIT(5), BIT(6)
 UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL, UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL = BIT(8), BIT(9)
+# hints in ucc_coll_args_t.flags (with UCC_COLL_ARGS_FIELD_FLAGS); tl/nvl honours OVERLAP_GPU (docs/user_guide.md)
+(UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_CPU, UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU,
+ UCC_COLL_ARGS_HINT_OPTIMIZE_LATENCY) = BIT(24), BIT(25), BIT(26)
 
 UCC_EE_CUDA_STREAM, UCC_EE_CPU_THREAD = 0, 1
 UCC_EVENT_COLLECTIVE_POST, UCC_EVENT_COLLECTIVE_COMPLETE, UCC_EVENT_COMPUTE_COMPLETE = BIT(0), BIT(1), BIT(2)

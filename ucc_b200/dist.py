@@ -166,6 +166,14 @@ def _relaxed_capture():
         _cu_capture_mode(C.byref(mode))
 
 
+def _overlap(a, on):
+    """mark a request with UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU"""
+    if on:
+        a.mask |= U.UCC_COLL_ARGS_FIELD_FLAGS
+        a.flags |= U.UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU
+    return a
+
+
 class Request:
     def __init__(self, comm, req, keep):
         self.comm, self.req, self._keep = comm, req, keep
@@ -499,16 +507,20 @@ class Communicator:
             imported.append(h)
         return MemHandles(self, tensor, local, imported, blobs)
 
-    def allreduce_init(self, src, dst, op="sum", persistent=False):
+    def allreduce_init(self, src, dst, op="sum", persistent=False, overlap_gpu=False):
         inplace = src is None or src.data_ptr() == dst.data_ptr()
         s = None if inplace else src
-        return self._init_cached(self._graph_key("allreduce", s, dst, {"op": op}),
-                                 lambda p: self._args("allreduce", s, dst, op=op, inplace=inplace, persistent=persistent or p), (src, dst))
 
-    def coll_init(self, coll, src=None, dst=None, src_memh=None, dst_memh=None, **kw):
-        """`src_memh` / `dst_memh`: MemHandles from register() - the buffers are parts of registered segments"""
+        def make(p):
+            return _overlap(self._args("allreduce", s, dst, op=op, inplace=inplace, persistent=persistent or p), overlap_gpu)
+        return self._init_cached(self._graph_key("allreduce", s, dst, {"op": op, "overlap_gpu": bool(overlap_gpu)}), make, (src, dst))
+
+    def coll_init(self, coll, src=None, dst=None, src_memh=None, dst_memh=None, overlap_gpu=False, **kw):
+        """`src_memh` / `dst_memh`: MemHandles from register() - the buffers are parts of registered segments.
+        `overlap_gpu`: the request carries UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU - on tl/nvl, data crosses NVLink by the copy
+        engines and the SMs stay free for kernels that run next to the collective (docs/user_guide.md)"""
         def make(persistent):
-            a = self._args(coll, src, dst, **dict(kw, persistent=kw.get("persistent", False) or persistent))
+            a = _overlap(self._args(coll, src, dst, **dict(kw, persistent=kw.get("persistent", False) or persistent)), overlap_gpu)
             if src_memh is not None:
                 a.mask |= U.UCC_COLL_ARGS_FIELD_MEM_MAP_SRC_MEMH | U.UCC_COLL_ARGS_FIELD_FLAGS
                 a.flags |= U.UCC_COLL_ARGS_FLAG_SRC_MEMH_GLOBAL
@@ -518,7 +530,7 @@ class Communicator:
                 a.flags |= U.UCC_COLL_ARGS_FLAG_DST_MEMH_GLOBAL
                 a.dst_memh.global_memh = C.cast(dst_memh.array, C.POINTER(C.c_void_p))
             return a
-        key = self._graph_key(coll, src, dst, dict(kw, src_memh=id(src_memh), dst_memh=id(dst_memh)))
+        key = self._graph_key(coll, src, dst, dict(kw, src_memh=id(src_memh), dst_memh=id(dst_memh), overlap_gpu=bool(overlap_gpu)))
         return self._init_cached(key, make, (src, dst, src_memh, dst_memh))
 
     def run(self, req, stream=None):

@@ -59,9 +59,11 @@ def _launch(comm, req, tensor, async_op, keep=(), wait_posted=True):
     return w
 
 
-def all_reduce(tensor, op="sum", comm=None, async_op=False):
+def all_reduce(tensor, op="sum", comm=None, async_op=False, overlap_gpu=False):
+    """`overlap_gpu` (every collective below has it): the request carries UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU, so tl/nvl moves
+    its data by the copy engines and leaves the SMs to the kernels that run next to it (docs/user_guide.md)"""
     comm = comm or default_comm()
-    return _launch(comm, comm.allreduce_init(tensor, tensor, op=op), tensor, async_op)
+    return _launch(comm, comm.allreduce_init(tensor, tensor, op=op, overlap_gpu=overlap_gpu), tensor, async_op)
 
 
 _from_host_state = {"chunks": 1}
@@ -117,42 +119,43 @@ def all_reduce_from_host(host, out, staging=None, op="sum", comm=None, chunks=No
     return out
 
 
-def reduce(tensor, dst=0, op="sum", comm=None, async_op=False):
+def reduce(tensor, dst=0, op="sum", comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
-    req = comm.coll_init("reduce", None if comm.rank == dst else tensor, tensor if comm.rank == dst else None, op=op, root=dst, inplace=comm.rank == dst)
+    req = comm.coll_init("reduce", None if comm.rank == dst else tensor, tensor if comm.rank == dst else None, op=op, root=dst, inplace=comm.rank == dst,
+                         overlap_gpu=overlap_gpu)
     return _launch(comm, req, tensor, async_op)
 
 
-def broadcast(tensor, src=0, comm=None, async_op=False):
+def broadcast(tensor, src=0, comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
-    return _launch(comm, comm.coll_init("bcast", tensor, None, root=src), tensor, async_op)
+    return _launch(comm, comm.coll_init("bcast", tensor, None, root=src, overlap_gpu=overlap_gpu), tensor, async_op)
 
 
-def all_gather_into_tensor(output, input, comm=None, async_op=False):
+def all_gather_into_tensor(output, input, comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
     assert output.numel() == input.numel() * comm.size
-    return _launch(comm, comm.coll_init("allgather", input, output), input, async_op)
+    return _launch(comm, comm.coll_init("allgather", input, output, overlap_gpu=overlap_gpu), input, async_op)
 
 
-def reduce_scatter_tensor(output, input, op="sum", comm=None, async_op=False):
+def reduce_scatter_tensor(output, input, op="sum", comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
     assert input.numel() == output.numel() * comm.size
-    return _launch(comm, comm.coll_init("reduce_scatter", input, output, op=op), input, async_op)
+    return _launch(comm, comm.coll_init("reduce_scatter", input, output, op=op, overlap_gpu=overlap_gpu), input, async_op)
 
 
-def all_to_all_single(output, input, output_split_sizes=None, input_split_sizes=None, comm=None, async_op=False):
+def all_to_all_single(output, input, output_split_sizes=None, input_split_sizes=None, comm=None, async_op=False, overlap_gpu=False):
     """Equal splits -> alltoall; explicit split sizes (in elements of dim 0 rows) -> alltoallv (MoE dispatch / combine)."""
     comm = comm or default_comm()
-    return _launch(comm, _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes), input, async_op)
+    return _launch(comm, _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes, overlap_gpu), input, async_op)
 
 
-def _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes):
+def _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes, overlap_gpu=False):
     """alltoall / alltoallv request; `output` and `input` being the same memory makes it an in-place request, whose counts and
     displacements are those of the output (an in-place alltoallv needs the same split sizes in both directions)"""
     inplace = output.data_ptr() == input.data_ptr()
     src = None if inplace else input
     if output_split_sizes is None and input_split_sizes is None:
-        return comm.coll_init("alltoall", src, output, inplace=inplace)
+        return comm.coll_init("alltoall", src, output, inplace=inplace, overlap_gpu=overlap_gpu)
     row = input[0].numel() if input.dim() > 1 else 1
     sc = [int(s) * row for s in input_split_sizes]
     rc = [int(s) * row for s in output_split_sizes]
@@ -161,24 +164,24 @@ def _alltoall_init(comm, output, input, output_split_sizes, input_split_sizes):
     if inplace:
         if sc != rc:
             raise ValueError("in-place all_to_all_single needs input_split_sizes == output_split_sizes")
-        return comm.coll_init("alltoallv", None, output, inplace=True, dst_counts=rc, dst_displs=rd)
-    return comm.coll_init("alltoallv", input, output, src_counts=sc, src_displs=sd, dst_counts=rc, dst_displs=rd)
+        return comm.coll_init("alltoallv", None, output, inplace=True, dst_counts=rc, dst_displs=rd, overlap_gpu=overlap_gpu)
+    return comm.coll_init("alltoallv", input, output, src_counts=sc, src_displs=sd, dst_counts=rc, dst_displs=rd, overlap_gpu=overlap_gpu)
 
 
-def all_gather_v(output, input, counts, comm=None, async_op=False):
+def all_gather_v(output, input, counts, comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
     displs = [sum(counts[:i]) for i in range(len(counts))]
-    return _launch(comm, comm.coll_init("allgatherv", input, output, dst_counts=list(counts), dst_displs=displs), input, async_op)
+    return _launch(comm, comm.coll_init("allgatherv", input, output, dst_counts=list(counts), dst_displs=displs, overlap_gpu=overlap_gpu), input, async_op)
 
 
-def gather(output, input, dst=0, comm=None, async_op=False):
+def gather(output, input, dst=0, comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
-    return _launch(comm, comm.coll_init("gather", input, output if comm.rank == dst else None, root=dst), input, async_op)
+    return _launch(comm, comm.coll_init("gather", input, output if comm.rank == dst else None, root=dst, overlap_gpu=overlap_gpu), input, async_op)
 
 
-def scatter(output, input, src=0, comm=None, async_op=False):
+def scatter(output, input, src=0, comm=None, async_op=False, overlap_gpu=False):
     comm = comm or default_comm()
-    return _launch(comm, comm.coll_init("scatter", input if comm.rank == src else None, output, root=src), output, async_op)
+    return _launch(comm, comm.coll_init("scatter", input if comm.rank == src else None, output, root=src, overlap_gpu=overlap_gpu), output, async_op)
 
 
 def barrier(comm=None):

@@ -160,6 +160,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         self._p2p_streams = {}
         self._coalesced = None   # between _start_coalescing and _end_coalescing: the Work of every operation
         self._name, self._desc = None, None
+        self._overlap_gpu = False
 
     def getBackendName(self):
         return "ucc_b200"
@@ -189,6 +190,16 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     def release_graphed(self):
         self._comm.release_graphed()
+
+    def set_overlap_gpu(self, on=True):
+        """Every collective of this group from now on carries UCC_COLL_ARGS_HINT_OPTIMIZE_OVERLAP_GPU (send / recv does not): on tl/nvl
+        its data crosses NVLink by the copy engines and the SMs stay free for the kernels that run next to it, e.g. the compute of
+        FSDP2 or DDP, whose group is `mesh.get_group()` / the process group passed to DDP.  Every member sets the same value, before
+        the same collective.  Results are bitwise those of the group without it (docs/user_guide.md)."""
+        self._overlap_gpu = bool(on)
+
+    def _init(self, coll, src=None, dst=None, **kw):
+        return self._comm.coll_init(coll, src, dst, overlap_gpu=self._overlap_gpu, **kw)
 
     # ---- helpers
     def _run(self, reqs, tensors, result, wait_posted=True, outs=(), views=()):
@@ -233,7 +244,7 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     # ---- collectives (list-of-tensors signatures of c10d)
     def allreduce(self, tensors, opts=None):
         op = _reduce_op(opts, tensors)
-        reqs = [self._comm.allreduce_init(t, t, op=op) for t in tensors]
+        reqs = [self._comm.allreduce_init(t, t, op=op, overlap_gpu=self._overlap_gpu) for t in tensors]
         return self._run(reqs, tensors, tensors)
 
     def allreduce_coalesced(self, tensors, opts=None):
@@ -241,14 +252,14 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
 
     def broadcast(self, tensors, opts=None):
         root = opts.rootRank if opts is not None else 0
-        reqs = [self._comm.coll_init("bcast", t, None, root=root) for t in tensors]
+        reqs = [self._init("bcast", t, None, root=root) for t in tensors]
         return self._run(reqs, tensors, tensors)
 
     def reduce(self, tensors, opts=None):
         root = opts.rootRank if opts is not None else 0
         op = _reduce_op(opts, tensors)
         me = self.rank()
-        reqs = [self._comm.coll_init("reduce", None if me == root else t, t if me == root else None, op=op, root=root, inplace=me == root) for t in tensors]
+        reqs = [self._init("reduce", None if me == root else t, t if me == root else None, op=op, root=root, inplace=me == root) for t in tensors]
         return self._run(reqs, tensors, tensors)
 
     # The list forms of allgather and reduce_scatter hold one block per rank, and every rank passes the whole list, so every rank
@@ -260,12 +271,12 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
             counts = [t.numel() for t in blocks]
             if len(set(counts)) == 1:
                 flat = torch.empty((len(blocks),) + tuple(inp.shape), dtype=inp.dtype, device=inp.device)
-                reqs.append(self._comm.coll_init("allgather", inp.contiguous(), flat))
+                reqs.append(self._init("allgather", inp.contiguous(), flat))
                 views += list(flat)
             else:
                 flat = _flat(sum(counts), inp)
                 src = inp.contiguous() if inp.numel() else _pack([inp])
-                reqs.append(self._comm.coll_init("allgatherv", src, flat, dst_counts=counts, dst_displs=_displs(counts)))
+                reqs.append(self._init("allgatherv", src, flat, dst_counts=counts, dst_displs=_displs(counts)))
                 views += _views(flat, blocks)
             outs += blocks
         return self._run(reqs, input_tensors, output_lists, outs=outs, views=views)
@@ -275,18 +286,18 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         return self.allgather([list(blocks) for blocks in zip(*output_lists)], input_list, opts)
 
     def _allgather_base(self, output, input, opts=None):
-        return self._run([self._comm.coll_init("allgather", input.contiguous(), output)], [input], output)
+        return self._run([self._init("allgather", input.contiguous(), output)], [input], output)
 
     def allgather_into_tensor_coalesced(self, outputs, inputs, opts=None):
-        return self._run([self._comm.coll_init("allgather", i.contiguous(), o) for o, i in zip(outputs, inputs)], inputs, outputs)
+        return self._run([self._init("allgather", i.contiguous(), o) for o, i in zip(outputs, inputs)], inputs, outputs)
 
     def _reduce_scatter_base(self, output, input, opts=None):
         op = _reduce_op(opts, [input])
-        return self._run([self._comm.coll_init("reduce_scatter", input.contiguous(), output, op=op)], [input], output)
+        return self._run([self._init("reduce_scatter", input.contiguous(), output, op=op)], [input], output)
 
     def reduce_scatter_tensor_coalesced(self, outputs, inputs, opts=None):
         op = _reduce_op(opts, inputs)
-        return self._run([self._comm.coll_init("reduce_scatter", i.contiguous(), o, op=op) for o, i in zip(outputs, inputs)], inputs, outputs)
+        return self._run([self._init("reduce_scatter", i.contiguous(), o, op=op) for o, i in zip(outputs, inputs)], inputs, outputs)
 
     def reduce_scatter(self, outputs, input_lists, opts=None):
         op = _reduce_op(opts, outputs)
@@ -295,11 +306,11 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
             counts = [t.numel() for t in ins]
             if len(set(counts)) == 1:
                 flat = torch.cat([t.reshape(-1) for t in ins])
-                reqs.append(self._comm.coll_init("reduce_scatter", flat, out, op=op))
+                reqs.append(self._init("reduce_scatter", flat, out, op=op))
             else:
                 flat = _pack(ins)
                 dst = out if out.numel() else _flat(0, out)
-                reqs.append(self._comm.coll_init("reduce_scatterv", flat, dst, op=op, dst_counts=counts, dst_displs=_displs(counts)))
+                reqs.append(self._init("reduce_scatterv", flat, dst, op=op, dst_counts=counts, dst_displs=_displs(counts)))
             keep.append(flat)
         w = self._run(reqs, outputs, outputs)
         w._keep = keep
@@ -308,7 +319,8 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     def alltoall_base(self, output, input, output_split_sizes, input_split_sizes, opts=None):
         # an output aliasing the input makes it an in-place request
         equal = not output_split_sizes and not input_split_sizes
-        req = _alltoall_init(self._comm, output, input.contiguous(), None if equal else output_split_sizes, None if equal else input_split_sizes)
+        req = _alltoall_init(self._comm, output, input.contiguous(), None if equal else output_split_sizes, None if equal else input_split_sizes,
+                             self._overlap_gpu)
         return self._run([req], [input], output)
 
     # A rank cannot see the block sizes of the others (a gather's non-roots do not even see the root's list), so deciding between a
@@ -320,7 +332,8 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
     # new on every call, so inside graphed() the other ranks move their block through a new buffer, too.
     def alltoall(self, output_tensors, input_tensors, opts=None):
         dst = _flat(sum(t.numel() for t in output_tensors), output_tensors[0])
-        req = _alltoall_init(self._comm, dst, _pack(input_tensors), [t.numel() for t in output_tensors], [t.numel() for t in input_tensors])
+        req = _alltoall_init(self._comm, dst, _pack(input_tensors), [t.numel() for t in output_tensors], [t.numel() for t in input_tensors],
+                             self._overlap_gpu)
         return self._run([req], input_tensors, output_tensors, outs=output_tensors, views=_views(dst, output_tensors))
 
     def gather(self, output_tensors, input_tensors, opts=None):
@@ -330,12 +343,12 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
         for i, inp in enumerate(input_tensors):
             src = inp.contiguous() if inp.numel() and not self._comm._graphing else _pack([inp])
             if self.rank() != root:
-                reqs.append(self._comm.coll_init("gatherv", src, None, root=root))
+                reqs.append(self._init("gatherv", src, None, root=root))
                 continue
             blocks = output_tensors[i]
             counts = [t.numel() for t in blocks]
             flat = _flat(sum(counts), inp)
-            reqs.append(self._comm.coll_init("gatherv", src, flat, root=root, dst_counts=counts, dst_displs=_displs(counts)))
+            reqs.append(self._init("gatherv", src, flat, root=root, dst_counts=counts, dst_displs=_displs(counts)))
             outs += blocks
             views += _views(flat, blocks)
         return self._run(reqs, input_tensors, output_tensors, outs=outs, views=views)
@@ -351,10 +364,10 @@ class ProcessGroupUCCB200(dist.ProcessGroup):
                 outs.append(out)
                 views.append(dst.view(out.shape))
             if self.rank() != root:
-                reqs.append(self._comm.coll_init("scatterv", None, dst, root=root))
+                reqs.append(self._init("scatterv", None, dst, root=root))
                 continue
             counts = [t.numel() for t in input_tensors[i]]
-            reqs.append(self._comm.coll_init("scatterv", _pack(input_tensors[i]), dst, root=root, src_counts=counts, src_displs=_displs(counts)))
+            reqs.append(self._init("scatterv", _pack(input_tensors[i]), dst, root=root, src_counts=counts, src_displs=_displs(counts)))
         return self._run(reqs, output_tensors, output_tensors, outs=outs, views=views)
 
     # ---- coalescing (torch's _coalescing_manager with a device): one Work that completes every operation of the block
